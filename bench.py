@@ -29,23 +29,23 @@ import torch  # noqa: E402
 # Algorithmic work per 1024x2048 crop (SURVEY.md §8d / BASELINE.md §2, conv FLOPs = 2*MAC)
 TFLOP_PER_CROP = {"ocrnet.HRNet_Mscale": 10.53, "ocrnet.HRNet": 7.77, "deepv3.DeepV3PlusW38": 34.95}
 FWD_TFLOP_1X = 3.0546
-# Launch-level roofline of one train step per 1024x2048 crop: sum over the step's launches of max(FLOPs / sustained bf16
-# peak, bytes / HBM copy bandwidth), from the static trace of the real step program (tools/trace_step.py,
-# profiles/r1_step_roofline_model.txt; peaks of MEASURED_PEAKS.json: 1386.7 TFLOP/s, 6572.9 GB/s)
+# Launch-level roofline of one train step per 1024x2048 crop: sum over the step's launches of max(FLOPs / bf16 peak,
+# bytes / HBM bandwidth), from the static trace of the real step program (python -O tools/trace_step.py --bn-cells
+# --tflops 989 --gbs 3350: the H100 SXM data sheet's dense bf16 rate and HBM3 bandwidth)
 # BatchNorm at --gpus N > 1: per-GPU statistics unless --syncbn. Every reference script trains with syncbn: true and the
 # NVLink exchange is validated and measured at N = 2 (tests/test_gpu_multi.py, DESIGN.md 6) - but never at N = 4 / 8 (the
 # round's GPU budget), so the driver's 1 -> 8 scaling runs use the configuration that is known to complete.
 SYNCBN_DEFAULT = False
-STEP_ROOFLINE_MS = {"ocrnet.HRNet_Mscale": 15.12, "ocrnet.HRNet": 11.34, "deepv3.DeepV3PlusW38": 30.8}
-# the same model per kernel class (profiles/r2_step_roofline_model.txt): class -> (kernel-name fragments, roofline ms)
+STEP_ROOFLINE_MS = {"ocrnet.HRNet_Mscale": 23.06, "ocrnet.HRNet": 17.27, "deepv3.DeepV3PlusW38": 43.9}
+# the same model per kernel class: class -> (kernel-name fragments, roofline ms)
 KERNEL_CLASSES = {
-    "conv fwd+dgrad (tcgen05)": (("conv3x3_halo", "conv_igemm"), 2.960 + 2.954 + 0.135),
-    "conv wgrad (tcgen05 + slab reduce)": (("wgrad_igemm", "wgrad_reduce"), 3.127),
-    "batchnorm passes": (("bn_",), 2.405 + 1.672 + 1.225),
-    "resample / fuse / accumulate": (("fuse_fwd", "upsample_adjoint", "masked_accum", "image_prep"), 0.359),
+    "conv fwd+dgrad (wgmma)": (("conv3x3_halo", "conv_igemm"), 4.206 + 4.750 + 0.610),
+    "conv wgrad (wgmma + slab reduce)": (("wgrad_igemm", "wgrad_reduce"), 5.285),
+    "batchnorm passes": (("bn_",), 4.719 + 2.177 + 0.239),
+    "resample / fuse / accumulate": (("fuse_fwd", "upsample_adjoint", "masked_accum", "image_prep"), 0.706),
     "loss + OCR softmaxes": (("loss_fwd", "_bwd_kernel", "mid_fwd", "softmax", "spatial_", "count_valid", "colsum",
-                              "cast_rows", "transpose_pad", "rmi_"), 0.19),
-    "weights / gradients / optimizer": (("pack_weights", "grad_fold", "publish_grads", "sgd_step", "running_update"), 0.27 + 0.8),
+                              "cast_rows", "transpose_pad", "rmi_"), 0.366),
+    "weights / gradients / optimizer": (("pack_weights", "grad_fold", "publish_grads", "sgd_step", "running_update"), 0.53 + 1.57),
 }
 
 
@@ -126,6 +126,8 @@ def parse():
                          "`vs_torch_gpu` to the line. Default at --gpus 1; this flag forces it for N > 1 (rank 0)")
     ap.add_argument("--no-torch-gpu-baseline", action="store_true")
     ap.add_argument("--no-recipe", action="store_true", help="skip the second (RMI + supervised multi-scale) measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (see dump_outputs)")
     return ap.parse_args()
 
 
@@ -136,11 +138,11 @@ def peaks():
             p = json.load(f)
         return dict(hbm_gbs=p["hbm_gbs"], tf_burst=p["bf16_tflops"], tf_sust=p.get("bf16_tflops_sustained",
                                                                                      p["bf16_tflops"]), src="measured")
-    return dict(hbm_gbs=6650.0, tf_burst=1590.0, tf_sust=1400.0, src="fallback")
+    return dict(hbm_gbs=3350.0, tf_burst=989.0, tf_sust=989.0, src="H100 SXM data sheet (700 W)")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     def __init__(self, index):
         self.index = index
@@ -334,23 +336,20 @@ def dominant_kernel_roofline(pk):
     t = ms[len(ms) // 2]
     flops = 2.0 * 256 * 512 * 720 * 512 * 9
     achieved = flops / (t * 1e-3) / 1e12
-    # DRAM traffic of this launch from the committed `ncu --set full` capture (profiles/r1_ncu_full_prof_ocr.txt:
-    # dram__bytes_read.sum 195.6 MB + dram__bytes_write.sum 100.6 MB); algorithmic bytes = in + out + weights in bf16
+    # algorithmic bytes = in + out + weights in bf16
     algo_bytes = 2.0 * (256 * 512 * 720 + 256 * 512 * 512 + 512 * 720 * 9)
     return dict(bound="tensor", kernel="conv3x3_halo_kernel (conv3x3_ocr 720->512 3x3 @256x512, bf16, fp32 accum, "
                                        "BN statistics in the epilogue)",
                 achieved=achieved, peak=pk["tf_burst"], unit="TFLOP/s", frac=achieved / pk["tf_burst"],
                 peak_source=pk["src"] + " bf16_tflops (burst: kernel timed alone)", ms_per_launch=t,
-                traffic=296.26e6, traffic_unit="bytes/launch (ncu dram read+write)",
-                traffic_source="profiles/r1_ncu_full_prof_ocr.txt (one ncu --set full capture of this launch; not "
-                               "re-measured in this run)", algorithmic_bytes=algo_bytes,
-                note="the largest single launch (1.4 % of the step); whole-step figures: model_flops_utilisation, "
-                     "step_roofline and kernel_classes")
+                algorithmic_bytes=algo_bytes,
+                note="the largest single launch; whole-step figures: model_flops_utilisation, step_roofline and "
+                     "kernel_classes")
 
 
 def time_dominant_kernel_roofline(pk):
-    """The kernel that takes the largest share of the step (profiles/r2_launch_summary_step_final.txt: conv3x3_halo_kernel<2>,
-    21.6 % of the serialised kernel time, 851 launches) on its most expensive instance: the 48 -> 48 3x3 convolution of the
+    """The halo convolution, the kernel with the most launches of the step (kernel_classes shows its share), on its most
+    expensive instance: the 48 -> 48 3x3 convolution of the
     high-resolution branch at 256x512 (64 forward launches + their data gradients per 1.0x pass). HBM-bound: algorithmic
     bytes = (in + out) x 2 B + weights = 25.2 MB per launch (SURVEY 8d per-conv figure). Timed alone with CUDA events on the
     launching stream, L2 flushed between iterations by writing a 256 MB buffer."""
@@ -377,17 +376,32 @@ def time_dominant_kernel_roofline(pk):
     algo_bytes = 2.0 * (2 * h * w * c + c * c * 9)
     achieved = algo_bytes / (t * 1e-3) / 1e9
     return dict(bound="hbm", kernel="conv3x3_halo_kernel<2> (48->48 3x3 @256x512 of the high-resolution HRNet branch, bf16, "
-                                    "fp32 accumulate in TMEM, BN statistics in the epilogue)",
+                                    "fp32 accumulate in registers, BN statistics in the epilogue)",
                 achieved=achieved, peak=pk["hbm_gbs"], unit="GB/s", frac=achieved / pk["hbm_gbs"],
                 peak_source=pk["src"] + " hbm_gbs (copy bandwidth)", ms_per_launch=t,
-                traffic=12.70e6, traffic_unit="bytes/launch (ncu dram read+write)",
-                traffic_source="profiles/r2_ncu_full_final.txt (ncu --set full of this launch: 12.70 MB read, the 12.6 MB "
-                               "output stays in the 126 MB L2 at kernel end; not re-measured in this run)",
                 algorithmic_bytes=algo_bytes,
-                note="the kernel with the largest share of the step (21.6 % of the serialised kernel time); latency bound "
-                     "with two resident CTAs per SM: tensor pipe ~11 %, DRAM ~7 % busy (DESIGN.md 7 gap 1). The largest "
-                     "single launch is in roofline_largest_launch; whole-step figures: model_flops_utilisation, "
-                     "step_roofline and kernel_classes")
+                note="the largest single launch is in roofline_largest_launch; whole-step figures: "
+                     "model_flops_utilisation, step_roofline and kernel_classes")
+
+
+def dump_outputs(out_dir, net, loss):
+    """What the timed step hands its caller: the loss, the gradients and the parameters after the optimizer step. The
+    gradients and parameters are a fixed seeded sample (same indices in every run) so the files stay below 64 MB."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    params = [p for _, p in net.named_parameters()]
+    grads = torch.cat([(p.grad if p.grad is not None else torch.zeros_like(p)).detach().float().reshape(-1)
+                       for p in params])
+    values = torch.cat([p.detach().float().reshape(-1) for p in params])
+    n = min(grads.numel(), 4 << 20)
+    idx = torch.randperm(grads.numel(), generator=torch.Generator().manual_seed(1234))[:n].sort().values
+    idx = idx.to(grads.device)
+    arrays = dict(loss=np.array([float(loss)], dtype=np.float64),
+                  grad_sample=grads[idx].cpu().numpy(), param_sample=values[idx].cpu().numpy(),
+                  grad_norms=np.array([float(p.grad.double().norm()) if p.grad is not None else 0.0 for p in params],
+                                      dtype=np.float64))
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def run_b200(args):
@@ -462,6 +476,8 @@ def run_b200(args):
     e1.record()
     barrier()
     ms = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, net, loss)
     if os.environ.get("B200SEG_TIME_ONLY") == "1":              # A/B runs of a switch: the device-timed figure only
         if rank == 0:
             print(json.dumps(dict(ms_per_step=ms / args.steps, steps=args.steps, time_only=True)))
@@ -554,7 +570,7 @@ def run_b200(args):
                               "finaliser, one-warp waiter kernels)" if (world > 1 and args.syncbn) else
                               "statistics local to each GPU" + (" (--no-syncbn)" if world > 1 else ""),
                     global_batch=B * world, parallelism="dp%d" % world, cuda_graph=not args.no_graph,
-                    l2_policy="per-step working set (>4 GB of activations) far exceeds the 126 MB L2; the "
+                    l2_policy="per-step working set (>4 GB of activations) far exceeds the 50 MB L2; the "
                               "single-kernel roofline run flushes L2 with a 256 MB write between iterations",
                     model_tflop_per_crop=TFLOP_PER_CROP[args.arch]),
         e2e=dict(value=e2e_value, unit="crops/s", ms_per_step=ms_e2e / args.steps,
@@ -577,7 +593,7 @@ def run_b200(args):
         step_roofline=dict(model_ms_per_step=STEP_ROOFLINE_MS[args.arch] * (H * W) / (1024.0 * 2048.0) * B,
                            frac=STEP_ROOFLINE_MS[args.arch] * (H * W) / (1024.0 * 2048.0) * B / (ms / args.steps),
                            what="sum over the step's launches of max(FLOPs/P, bytes/B), static trace of the step "
-                                "program (profiles/r1_step_roofline_model.txt)"),
+                                "program (tools/trace_step.py, H100 data-sheet peaks)"),
         roofline=roof, roofline_largest_launch=largest, kernel_classes=classes, clocks=clocks, last_loss=loss_val,
         max_memory_allocated_gb=round(torch.cuda.max_memory_allocated() / 2 ** 30, 2))
     if world == 1 and not args.no_recipe and args.criterion == "ce" and args.sup_wt == 0.0:

@@ -1,5 +1,5 @@
 /*
- * b200seg.h — C ABI of libb200seg.so: the sm_100a kernels behind the HRNet-OCR-MScale hot path of
+ * b200seg.h — C ABI of libb200seg.so: the sm_90a kernels behind the HRNet-OCR-MScale hot path of
  * NVIDIA/semantic-segmentation (reference @ /root/reference).
  *
  * Conventions (SURVEY.md §8b "What the C-ABI replacement must export"):
@@ -26,15 +26,15 @@ extern "C" {
 
 #define B200SEG_E_BADARG (-1)      /* shape / alignment not supported by the kernel */
 #define B200SEG_E_NODRIVER (-100)  /* cuTensorMapEncodeTiled entry point unavailable */
-#define B200SEG_MAX_CTAS 148       /* SMs of a B200 */
-#define B200SEG_MAX_GRID 296       /* persistent grids: at most two co-resident CTAs per SM (narrow Cout tiles) */
+#define B200SEG_MAX_CTAS 132       /* SMs of an H100 SXM */
+#define B200SEG_MAX_GRID 264       /* persistent grids: at most two co-resident CTAs per SM (narrow Cout tiles) */
 
 /* ABI / build identification. */
 int b200seg_abi_version(void);
 const char* b200seg_build_info(void);
 
 /* ------------------------------------------------------------------------------------------------
- * Convolution as implicit GEMM on tcgen05 (TMA-fed, TMEM accumulators).
+ * Convolution as implicit GEMM on wgmma (TMA-fed, register accumulators).
  * Replaces cuDNN behind nn.Conv2d at network/hrnetv2.py:31-34,74-80,193-198,208-210,270-274,
  * network/ocrnet.py:54-57,66-76, network/ocr_utils.py:68-91,142-144, network/utils.py:348-362.
  * ------------------------------------------------------------------------------------------------ */
@@ -56,7 +56,7 @@ typedef struct b200seg_conv_desc {
 
 /* Host-only introspection of the launch plan (tests, tuning): which = 0 forward, 1 stride-1 data gradient.
  * out[10] = {kernel (1 = halo-tile 3x3, 0 = per-tap implicit GEMM), Cout tile, Cout tiles, grid, dynamic shared memory
- * bytes, ring depth, CTAs per SM, TMEM columns, resident weights, weight slots}. Returns 0 or a negative error. */
+ * bytes, ring depth, CTAs per SM, accumulator registers per thread, resident weights, weight slots}. Returns 0 or a negative error. */
 int b200seg_conv2d_plan_info(const b200seg_conv_desc* d, int32_t which, int32_t* out);
 
 /* Diagnostics (needs a GPU): CTAs per SM the runtime grants kernel (1 = halo-tile 3x3, 0 = per-tap) in its
@@ -149,7 +149,7 @@ int b200seg_pack_weights(const b200seg_pack_item* items, const int32_t* blk_item
 /* Data gradient: dx[n,h,w,cin] = conv_transpose(dy, W) (+ addend, e.g. a gradient that already arrived at x).
  * d describes the FORWARD convolution; dy: bf16 [n,ho,wo,*] whose channel extent is roundup8(cout) (pad channels
  * zero); w_dgrad from b200seg_pack_weight with o_pad = roundup8(cout). Stride-2 convolutions run as four parity-class
- * launches of the same tcgen05 kernel. Replaces cuDNN convolution_backward (input part). */
+ * launches of the same wgmma kernel. Replaces cuDNN convolution_backward (input part). */
 int b200seg_conv2d_dgrad(const b200seg_conv_desc* d, const void* dy, int32_t dy_ld, const void* w_dgrad,
                          const void* addend, int32_t addend_ld, void* dx, int32_t dx_ld, void* stream);
 
@@ -157,7 +157,7 @@ int b200seg_conv2d_dgrad(const b200seg_conv_desc* d, const void* dy, int32_t dy_
 /* Weight gradient: dw_ohwi[co][kh*kw][ci] (fp32 accumulator in the kernels' own layout, 16-byte aligned)
  *   += sum_pixels dy[.., co] * x_shifted[.., ci]        (the convolution weight gradient, SURVEY.md K1-K5).
  * d describes the FORWARD convolution (input geometry, stride, pad); dy is bf16 NHWC [n,ho,wo,cout] with pitch dy_ld;
- * cin multiple of 16. Deterministic. Depending on the shape the tcgen05 kernel either owns every gradient element
+ * cin multiple of 16. Deterministic. Depending on the shape the wgmma kernel either owns every gradient element
  * (one launch, no workspace) or writes per-work-unit fp32 slabs into the caller's workspace that a second kernel sums
  * in a fixed order; _ws_bytes / _launches report which. b200seg_grad_fold turns the accumulators into OIHW gradients. */
 size_t b200seg_conv2d_wgrad_ws_bytes(const b200seg_conv_desc* d);

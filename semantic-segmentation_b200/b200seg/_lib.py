@@ -66,19 +66,6 @@ class AugColor(ctypes.Structure):
                 ("mean", c_float * 3), ("std", c_float * 3)]
 
 
-class ProbeOperand(ctypes.Structure):
-    _fields_ = [(n, c_int32) for n in (
-        "rows", "cols", "box_cols", "box_rows", "nboxes", "c0", "r0", "dcol", "drow", "smem_stride",
-        "swizzle_bytes")]
-
-
-class ProbeDesc(ctypes.Structure):
-    _fields_ = [("a", ProbeOperand), ("b", ProbeOperand)] + [(n, c_int32) for n in (
-        "M", "N", "ksteps",
-        "a_off", "a_lbo", "a_sbo", "a_layout", "a_base", "a_major", "a_kstep",
-        "b_off", "b_lbo", "b_sbo", "b_layout", "b_base", "b_major", "b_kstep")]
-
-
 # name -> (restype, argtypes). Must list every symbol include/b200seg.h declares (tests/test_abi.py checks this).
 V, I32, I64, F = c_void_p, c_int32, c_int64, c_float
 SIGNATURES = {
@@ -165,7 +152,6 @@ SIGNATURES = {
 # test-only entry points (csrc/probe.h, libb200seg_test.so), not part of include/b200seg.h / the product library
 PROBE_SIGNATURES = {
     "b200seg_conv2d_fwd_direct": (ctypes.c_int, [ctypes.POINTER(ConvDesc), V, V, V, V, V]),
-    "b200seg_umma_probe": (ctypes.c_int, [ctypes.POINTER(ProbeDesc), V, V, V, V]),
 }
 
 _lib = None
@@ -197,7 +183,7 @@ _test_lib = None
 
 
 def test_lib():
-    """The test-only library (direct cross-check convolution, descriptor probe); never loaded by the product path."""
+    """The test-only library (direct cross-check convolution); never loaded by the product path."""
     global _test_lib
     if _test_lib is None:
         if not os.path.exists(TEST_LIB_PATH):

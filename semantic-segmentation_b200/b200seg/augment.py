@@ -6,7 +6,7 @@
     -> ToTensor -> Normalize (datasets/__init__.py:102-104) and MaskToTensor, after the label-id remap of
     datasets/base_loader.py:177-181
 
-as three sm_100a kernels (csrc/augment_kernels.cu) on the DECODED uint8 frame, so a 1024x2048 crop costs microseconds on
+as three sm_90a kernels (csrc/augment_kernels.cu) on the DECODED uint8 frame, so a 1024x2048 crop costs microseconds on
 the GPU instead of a PIL worker process per GPU. Results are bit-exact with PIL 12 on the uint8 stages and with
 torchvision's ToTensor / Normalize arithmetic on the fp32 stage (tests/test_gpu_augment.py): the host side below draws
 the random parameters with the reference's own generator calls in the reference's order (`random` for the geometry,

@@ -7,7 +7,7 @@ Design notes
   * ``Act`` is an NHWC bf16 activation (possibly a channel-slice view of a wider buffer, so concat is a no-op).
     ``Act.grad`` accumulates in place: producers of a gradient either create it or pass the existing buffer as the
     kernel's addend.
-  * conv -> training BatchNorm -> (residual) -> ReLU is three passes: the tcgen05 conv emits the batch statistics from
+  * conv -> training BatchNorm -> (residual) -> ReLU is three passes: the wgmma conv emits the batch statistics from
     its epilogue, ``bn_finalize`` turns them into scale/shift (+ running stats), ``bn_apply`` fuses affine, residual,
     ReLU and the Dropout2d mask. The backward mirrors it (``bn_bwd`` = reduce + finalize + apply, then wgrad, dgrad).
 """

@@ -1,4 +1,4 @@
-"""Eval-mode forward: per-scale passes on the sm_100a kernels (BatchNorm from running statistics, no tape), then the
+"""Eval-mode forward: per-scale passes on the sm_90a kernels (BatchNorm from running statistics, no tape), then the
 reference's output assembly in fp32 NCHW on the device.
 
   ocrnet.HRNet_Mscale : MscaleOCR.nscale_forward when cfg.MODEL.N_SCALES is set (network/ocrnet.py:185-262), else the

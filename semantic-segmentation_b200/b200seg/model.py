@@ -112,7 +112,7 @@ def hrnet_forward(E, x16, hcfg, p="backbone"):
 # ----------------------------------------------------------------------------------------------- OCR head
 def spatial_gather(E, feats, aux, K):
     """SpatialGather_Module.forward (network/ocr_utils.py:34-46): context[n,k,:] = sum_pix softmax_pix(aux)[pix,k] *
-    feats[pix,:]. The softmax runs over pixels; the product is the tcgen05 weight-gradient GEMM (pixels = reduction).
+    feats[pix,:]. The softmax runs over pixels; the product is the wgmma weight-gradient GEMM (pixels = reduction).
     feats: Act [n,h,w,C]; aux: HeadRec with fp32 logits. Returns the proxy Act [n,K,1,C] (bf16)."""
     n, h, w, C = feats.t.shape
     P = h * w

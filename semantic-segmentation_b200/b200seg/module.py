@@ -101,7 +101,7 @@ class B200SegModule(nn.Module):
         self.parallel_branches = parallel_branches  # HRNet branches of a module on parallel streams
         # SyncBN (config.py:216-225, every scripts/*.yml sets syncbn: true): True = statistics of the global batch through
         # NVLink peer memory (needs torch.distributed, world > 1); None / False = per-GPU statistics. Opt-in for now: the
-        # exchange was validated on 2 GPUs only (DESIGN.md §6).
+        # exchange was validated on 2 GPUs only.
         self.syncbn = syncbn
         # BatchNorm statistics finalised inside the producing launches (csrc/bn_fold.cuh): 1262 launches fewer per step,
         # but measured 0.9 ms SLOWER on the device (40.18 vs 39.3 ms, alternating runs on one box: the tail of every
@@ -184,7 +184,7 @@ class B200SegModule(nn.Module):
         params = [(n, p) for n, p in self.named_parameters()]
         dev = params[0][1].device
         if dev.type != "cuda":
-            raise RuntimeError("B200SegModule runs on CUDA only (sm_100a); there is no CPU path - call .cuda() first")
+            raise RuntimeError("B200SegModule runs on CUDA only (sm_90a); there is no CPU path - call .cuda() first")
         if self._flat_grad is None or self._flat_grad.device != dev:
             total = sum((p.numel() + 63) // 64 * 64 for _, p in params)
             self._flat_grad = torch.zeros(total, dtype=F32, device=dev)      # published gradients (param.grad views)

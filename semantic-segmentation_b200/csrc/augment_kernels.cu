@@ -218,7 +218,7 @@ extern "C" int b200seg_aug_resize_crop(const b200seg_aug_geom* d, const uint8_t*
   g.ksize_v = d->ksize_v; g.ksize_h = d->ksize_h; g.flip = d->flip; g.ignore_label = d->ignore_label;
   const long long total = (long long)d->out_h * d->out_w;
   long long blocks = (total + 255) / 256;
-  if (blocks > 148LL * 16) blocks = 148LL * 16;
+  if (blocks > (long long)B200SEG_MAX_CTAS * 16) blocks = (long long)B200SEG_MAX_CTAS * 16;
   cudaError_t e = launch_k(aug_resize_crop_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, g, src_rgb,
                            src_mask, kk_h, bounds_h, kk_v, bounds_v, near_x, near_y, id_lut, out_rgb,
                            (long long*)out_label);
@@ -243,7 +243,7 @@ extern "C" int b200seg_aug_color_normalize(const b200seg_aug_color* c, const uin
   for (int i = 0; i < 3; ++i) { k.mean[i] = c->mean[i]; k.std[i] = c->std[i]; }
   const long long npix = (long long)h * w;
   long long blocks = (npix + 255) / 256;
-  if (blocks > 148LL * 16) blocks = 148LL * 16;
+  if (blocks > (long long)B200SEG_MAX_CTAS * 16) blocks = (long long)B200SEG_MAX_CTAS * 16;
   if (contrast_at >= 0) {
     if (!luma_sum_ws) return B200SEG_E_BADARG;
     cudaError_t e0 = cudaMemsetAsync(luma_sum_ws, 0, sizeof(uint64_t), (cudaStream_t)stream);

@@ -8,7 +8,7 @@
 // Deferred variant (counter == nullptr, the default of the training step): the CTAs only add their sums to the cells; the
 // BatchNorm apply pass that consumes the layer folds the totals in its prologue (b200seg_bn_apply_cells), so neither a
 // finaliser launch nor a last-CTA tail sits between the convolution and its consumer. The cells are zeroed by the caller
-// once per step. A sum of <= 296 fp32 partials in fp64 is exact unless their magnitudes differ by more than 2^20, so
+// once per step. A sum of <= B200SEG_MAX_GRID fp32 partials in fp64 is exact unless their magnitudes differ by more than 2^20, so
 // the order of the adds does not change the result in practice.
 #pragma once
 #include <cstdint>
@@ -36,13 +36,16 @@ struct BnFoldDev {
 // scale != nullptr): the epilogue stores relu?(acc * scale[c] + shift[c] (+ addend)) - one launch per conv + BN (+ residual)
 // + ReLU instead of three (b200seg_conv2d_fwd_affine). A convolution bias is folded into shift by the caller.
 
-// Called by ALL threads of the CTA after its last tile (s_stats = [4 quarters][2][cout_pad] per-CTA sums in shared memory,
+// Per-CTA statistics of a convolution: one [2][cout_pad] slot per epilogue warp (two warpgroups of four), summed in slot order.
+constexpr int kStatSlots = 8;
+// Called by ALL threads of the CTA after its last tile (s_stats = [kStatSlots][2][cout_pad] sums in shared memory,
 // already synchronised; s_ticket_p = one free word of the CTA's dynamic shared memory). Returns after the layer's parameters are written if this CTA drew the last ticket.
 __device__ __forceinline__ void bn_fold_tail(const BnFoldDev& f, const float* s_stats, int cout_pad,
                                              volatile unsigned* s_ticket_p) {
   const int nthreads = blockDim.x;
   for (int i = threadIdx.x; i < 2 * cout_pad; i += nthreads) {
-    const float v = (s_stats[i] + s_stats[2 * cout_pad + i]) + (s_stats[4 * cout_pad + i] + s_stats[6 * cout_pad + i]);
+    float v = 0.f;
+    for (int s = 0; s < kStatSlots; ++s) v += s_stats[2 * s * cout_pad + i];
     atomicAdd(f.accum + i, (double)v);
   }
   // Only the threads that added to the accumulator fence (their adds must be visible before the ticket is drawn): a

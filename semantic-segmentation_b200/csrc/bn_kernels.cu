@@ -1,4 +1,4 @@
-// Training-mode BatchNorm around the tcgen05 convolutions (reference: Norm2d -> torch.nn.BatchNorm2d /
+// Training-mode BatchNorm around the tensor-core convolutions (reference: Norm2d -> torch.nn.BatchNorm2d /
 // apex SyncBatchNorm, network/mynn.py:18-24; eps 1e-5, momentum 0.1, biased variance to normalise, unbiased for the
 // running estimate). All kernels are HBM-bound streaming passes over NHWC bf16 with 16-byte vector accesses.
 //
@@ -644,11 +644,11 @@ masked_accum_kernel(const __nv_bfloat16* __restrict__ src, int src_ld, const __n
 }
 
 // Grid of the element-wise passes: one 256-thread block per 256 x ew_items 16-byte items (the kernels keep several
-// independent items in flight per thread only when the grid leaves them more than one), capped at ew_ctas_per_sm x 148.
+// independent items in flight per thread only when the grid leaves them more than one), capped at ew_ctas_per_sm x SMs.
 static inline int ew_grid(long long total_threads) {
   const long long per = 256LL * (tune().ew_items > 0 ? tune().ew_items : 1);
   long long b = (total_threads + per - 1) / per;
-  const long long cap = 148LL * (tune().ew_ctas_per_sm > 0 ? tune().ew_ctas_per_sm : 8);
+  const long long cap = (long long)B200SEG_MAX_CTAS * (tune().ew_ctas_per_sm > 0 ? tune().ew_ctas_per_sm : 8);
   return (int)(b < cap ? (b > 0 ? b : 1) : cap);
 }
 
@@ -712,7 +712,7 @@ extern "C" int b200seg_accum_f32(float* dst, const float* src, int64_t n, void* 
   if (!dst || !src || n <= 0 || (n & 3) || (reinterpret_cast<uintptr_t>(dst) & 15) ||
       (reinterpret_cast<uintptr_t>(src) & 15))
     return B200SEG_E_BADARG;
-  launch_k(accum_f32_kernel, dim3(148 * 8), dim3(256), 0, (cudaStream_t)stream, dst, src, (long long)(n / 4));
+  launch_k(accum_f32_kernel, dim3(B200SEG_MAX_CTAS * 8), dim3(256), 0, (cudaStream_t)stream, dst, src, (long long)(n / 4));
   CHECK_LAUNCH();
 }
 
@@ -769,7 +769,7 @@ extern "C" int32_t b200seg_bn_bwd_grid(int64_t npix, int32_t c) {
   reduce_shape(c, &rows, &threads);
   const long long per = (long long)rows * (tune().red_items > 0 ? tune().red_items : 1);
   long long b = (npix + per - 1) / per;
-  const long long cap = 148LL * (tune().red_ctas_per_sm > 0 ? tune().red_ctas_per_sm : 2);
+  const long long cap = (long long)B200SEG_MAX_CTAS * (tune().red_ctas_per_sm > 0 ? tune().red_ctas_per_sm : 2);
   return (int32_t)(b < cap ? (b > 0 ? b : 1) : cap);
 }
 

@@ -2,16 +2,14 @@
 //
 // The generic kernel (conv_igemm.cu) fetches a shifted 128-pixel box per filter tap, i.e. it reads the input 9 times
 // from L2 — the limiter of HRNet's 48/96-channel high-resolution branch, which is HBM-bound on paper. Here the TMA unit
-// brings a (16+2) x (8+2) pixel halo tile (64-channel chunk, SWIZZLE_128B, 128 bytes per pixel row) into shared memory
-// ONCE, and the nine taps are nine tcgen05 shared-memory descriptors into that same tile:
-//     start = tile + (kh*10 + kw) * 128 B,   stride-byte-offset = 10 * 128 B (one 8-pixel tile row per 8-row group)
-// which works because the tensor core applies the 128B swizzle to absolute shared-memory addresses (pinned on silicon,
-// profiles/r1_umma_probe.txt: row-shifted starts and arbitrary SBO read exactly the rows TMA wrote).
+// brings a (16+2) x (8+2) pixel halo tile of a 64-channel chunk into shared memory ONCE, and the nine taps are nine
+// wgmma shared-memory descriptors into that same tile. The tile is stored without swizzle as eight planes of 8 channels
+// ([channel group][18][10][8 channels], 16 bytes per pixel of a plane, one TMA box of 8 channels per plane), so every
+// 8-pixel run of a plane is one 8 x 16-byte core matrix at any pixel offset:
+//     start = plane + (kh*10 + kw) * 16 B,   SBO = 10 * 16 B (next tile row),   LBO = plane pitch (next channel group)
+// The weights use the same no-swizzle layout ([channel group][BN][8 channels]).
 //
-// Roles (384 threads): warp 0 = TMA producer, warp 1 = ONE elected thread that waits on the barriers and issues every
-// tcgen05.mma of the CTA from fully unrolled code (a narrow layer's MMA lasts ~32 clocks, so the issue path must be a
-// handful of uniform-datapath instructions per MMA), warp 2 = TMEM allocator, warps 4-11 = epilogue: two warps per TMEM
-// lane quarter, each taking half of the accumulator columns.
+// Roles (288 threads): warps 0-7 = two consumer warpgroups (tile rows 0-7 / 8-15: MMA + epilogue), warp 8 = TMA producer.
 // Weights: resident in shared memory for the whole persistent CTA when they fit (C <= 96: the HBM-bound layers), else
 // streamed per (chunk, tap) through an mbarrier ring. The Cout tile (BN) is chosen per launch by a small cost model so
 // that low-resolution layers still spread over the SMs (a 16x32x384 layer has 4 pixel tiles but 6 x 64-wide Cout tiles).
@@ -21,10 +19,10 @@
 #include "ptx.cuh"
 #include "bn_fold.cuh"
 #include "conv_common.h"
+#include "conv_epi.cuh"
 #include "tma_host.h"
 #include "launch.h"
 #include "../../include/b200seg.h"
-#include "vec.cuh"
 #include <cstdlib>
 
 namespace b200seg {
@@ -39,125 +37,62 @@ struct HaloParams {
   int resident;                // weights stay in smem for the CTA lifetime
   int a_slots, b_slots;        // ring depths (b_slots unused when resident)
   int b_tile_bytes;            // BN * 128 rounded to 1024
-  int acc_stride, tmem_cols;   // TMEM: two accumulator buffers of acc_stride = pow2 >= BN columns (tmem_cols = 2 * acc_stride)
-  int dbg;                     // B200SEG_DBG=8: block 0 records a per-role ns timeline behind the statistics partials
-  int stage_bytes;             // FAST epilogue: two 16 KB output staging tiles behind the operand buffers, else 0
 };
 
-constexpr int kHThreads = 384;
-constexpr int kASlotBytes = 24576;     // 180 halo rows x 128 B = 23040, padded to a 1024 multiple
+constexpr int kHThreads = 288;
+constexpr int kASlotBytes = 24576;     // 8 planes x 2944 B = 23552, padded to a 1024 multiple
 constexpr int kHaloW = 10, kHaloH = 18, kTW = 8, kTH = 16;
+constexpr int kPlaneBytes = kHaloH * kHaloW * 16;   // one 8-channel plane of the halo tile (2880 B)
+constexpr int kPlane = 2944;                         // plane pitch: TMA destinations are 128-byte aligned
 constexpr int kMaxASlots = 4, kMaxBSlots2 = 8;
-constexpr int kStageTile = 128 * 128;  // 128 output pixels x 128 B (64 bf16 channels), SWIZZLE_128B like the operand tiles
 
-// Sum v[0..15] over the 32 lanes of the warp: afterwards v[0] holds the total for channel (lane & 15).
-__device__ __forceinline__ void h_butterfly16(float (&v)[16], uint32_t lane) {
-#pragma unroll
-  for (int off = 8; off >= 1; off >>= 1) {
-    const bool up = (lane & off) != 0;
-#pragma unroll
-    for (int i = 0; i < off; ++i) {
-      const float send = up ? v[i] : v[i + off];
-      const float keep = up ? v[i + off] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-    }
-  }
-  v[0] += __shfl_xor_sync(0xffffffffu, v[0], 16);
-}
-
-__device__ __forceinline__ unsigned long long gtime() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
-}
-// bench-only timeline (tools/gpu_timeline.py; build with EXTRA=-DB200SEG_TIMELINE): role r, tile iteration it -> ns
-#ifdef B200SEG_TIMELINE
-#define DBG_TS(role, it)                                                                                      \
-  do {                                                                                                        \
-    if ((p.dbg & 8) && blockIdx.x == 0 && (it) < 16)                                                          \
-      reinterpret_cast<unsigned long long*>(stats_partials + B200SEG_MAX_GRID * 2 * 1024)[(role) * 16 + (it)] = gtime();  \
-  } while (0)
-#else
-#define DBG_TS(role, it) do { } while (0)
-#endif
-
-// All nine taps of one resident 64-channel chunk: 9 x KS MMAs, compile-time offsets only.
-template <int KS>
-__device__ __forceinline__ void halo_issue9(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t btile16,
-                                            uint32_t idesc, uint32_t acc_first) {
-#pragma unroll
-  for (int t = 0; t < 9; ++t) {
-    const int kh = t / 3, kw = t - kh * 3;
-    const uint64_t ad = adesc + (uint64_t)((kh * kHaloW + kw) * 8);   // (kh*10 + kw) rows of 128 B, in 16-byte units
-#pragma unroll
-    for (int k = 0; k < KS; ++k)
-      umma_f16(d_tmem, ad + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc, (t | k) ? 1u : acc_first);
-    bdesc += btile16;
-  }
-}
-
-// OCC: CTAs per SM the register budget allows: 2 -> 80 registers (co-resident narrow tiles), 1 -> full register file.
-// FAST (narrow layers: one Cout tile of at most 64 channels, the HBM-bound ones; OCC = 1 only): the epilogue
-//   * stages the bf16 tile in shared memory (swizzled, conflict-free 16-byte stores) and writes it with ONE TMA store per
-//     tile (coalesced, clipped at the image edge by the tensor map) instead of 32-byte pieces at a 96-byte pitch per thread;
-//   * keeps the batch statistics of its pixel slot in registers across all tiles of the persistent CTA and reduces them
-//     across the warp ONCE at the end (two 16-way butterflies per 16 channels per TILE were ~1/2 of the epilogue time).
-template <int OCC, bool FAST>
+// OCC: CTAs per SM; the two-per-SM build holds at most 128 accumulator columns (64 registers per consumer thread).
+template <int OCC>
 __global__ void __launch_bounds__(kHThreads, OCC)
 conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                    const __grid_constant__ CUtensorMap tmY, const HaloParams p, __nv_bfloat16* __restrict__ y,
-                    const float* __restrict__ bias, float* __restrict__ stats_partials,
-                    const __nv_bfloat16* __restrict__ addend, const BnFoldDev fold) {
+                    const HaloParams p, __nv_bfloat16* __restrict__ y, const float* __restrict__ bias,
+                    float* __restrict__ stats_partials, const __nv_bfloat16* __restrict__ addend, const BnFoldDev fold) {
+  constexpr int NB = OCC == 2 ? 8 : 16;    // 16-column accumulator blocks
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* a_base = smem;
   uint8_t* b_base = smem + (size_t)p.a_slots * kASlotBytes;
   const int b_tiles_total = p.resident ? 9 * p.cchunks : p.b_slots;
-  uint8_t* stage_base = b_base + (size_t)b_tiles_total * p.b_tile_bytes;      // 1024-aligned (all tiles are)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(stage_base + p.stage_bytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(b_base + (size_t)b_tiles_total * p.b_tile_bytes);
   uint64_t* a_full = bars;                         // [kMaxASlots]
   uint64_t* a_empty = bars + kMaxASlots;
   uint64_t* b_full = bars + 2 * kMaxASlots;        // [kMaxBSlots2] (resident: only [0])
   uint64_t* b_empty = b_full + kMaxBSlots2;
-  uint64_t* tfull = b_empty + kMaxBSlots2;         // [2]
-  uint64_t* tempty = tfull + 2;                    // [2]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tempty + 2);
-  float* s_stats = reinterpret_cast<float*>(tmem_ptr_smem + 4);   // [4 lane quarters][2][cout_pad]
+  uint32_t* ticket = reinterpret_cast<uint32_t*>(b_empty + kMaxBSlots2);
+  float* s_stats = reinterpret_cast<float*>(ticket + 4);   // [kStatSlots][2][cout_pad]
 
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    if (FAST) tma_prefetch_desc(&tmY);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < p.a_slots; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 1); }
-    for (int s = 0; s < kMaxBSlots2; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tfull[s], 1); mbar_init(&tempty[s], 8); }
+    for (int s = 0; s < p.a_slots; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 2); }
+    for (int s = 0; s < kMaxBSlots2; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 2); }
     fence_barrier_init();
   }
-  if (warp == 2) { tmem_alloc(tmem_ptr_smem, p.tmem_cols); tmem_relinquish(); }
   if (p.emit_stats)
-    for (int i = threadIdx.x; i < 4 * 2 * p.cout_pad; i += kHThreads) s_stats[i] = 0.f;
-  tc_fence_before();
+    for (int i = threadIdx.x; i < kStatSlots * 2 * p.cout_pad; i += kHThreads) s_stats[i] = 0.f;
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   // Resident weights are static for the whole step (written by the pack kernels, which never trigger a programmatic
   // launch): fetch them while the previous kernel on the stream is still draining.
-  if (warp == 0 && p.resident) {
+  if (warp == 8 && p.resident) {
     if (elect_one()) {
       mbar_arrive_expect_tx(&b_full[0], 9 * p.cchunks * p.b_tile_bytes);
       for (int cc = 0; cc < p.cchunks; ++cc)
         for (int t = 0; t < 9; ++t)
-          tma_load_3d(&tmB, &b_full[0], b_base + (size_t)(cc * 9 + t) * p.b_tile_bytes, cc * 64, t, 0);
+          for (int j = 0; j < 8; ++j)
+            tma_load_3d(&tmB, &b_full[0], b_base + (size_t)(cc * 9 + t) * p.b_tile_bytes + j * p.BN * 16, cc * 64 + 8 * j,
+                        t, 0);
     }
     __syncwarp();
   }
   pdl_sync();   // everything above overlapped the previous kernel's tail; activations are touched only below
-  if (threadIdx.x == 0) DBG_TS(6, 0);
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ------------------------------------------------------------------ TMA producer (one elected lane)
     if (elect_one()) {
       int a_slot = 0, b_slot = 0;
@@ -169,16 +104,18 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         const int img = m_tile / (p.tiles_w * p.tiles_h);
         for (int cc = 0; cc < p.cchunks; ++cc) {
           mbar_wait(&a_empty[a_slot], a_phase ^ 1);
-          mbar_arrive_expect_tx(&a_full[a_slot], kHaloH * kHaloW * 128);
-          tma_load_4d(&tmA, &a_full[a_slot], a_base + (size_t)a_slot * kASlotBytes, cc * 64, tw_i * kTW - 1,
-                      th_i * kTH - 1, img);
-          DBG_TS(0, (tile - (int)blockIdx.x) / (int)gridDim.x);
+          mbar_arrive_expect_tx(&a_full[a_slot], 8 * kPlaneBytes);
+          for (int j = 0; j < 8; ++j)
+            tma_load_4d(&tmA, &a_full[a_slot], a_base + (size_t)a_slot * kASlotBytes + j * kPlane, cc * 64 + 8 * j,
+                        tw_i * kTW - 1, th_i * kTH - 1, img);
           if (++a_slot == p.a_slots) { a_slot = 0; a_phase ^= 1; }
           if (!p.resident) {
             for (int t = 0; t < 9; ++t) {
               mbar_wait(&b_empty[b_slot], b_phase ^ 1);
               mbar_arrive_expect_tx(&b_full[b_slot], p.b_tile_bytes);
-              tma_load_3d(&tmB, &b_full[b_slot], b_base + (size_t)b_slot * p.b_tile_bytes, cc * 64, t, n_tile * p.BN);
+              for (int j = 0; j < 8; ++j)
+                tma_load_3d(&tmB, &b_full[b_slot], b_base + (size_t)b_slot * p.b_tile_bytes + j * p.BN * 16,
+                            cc * 64 + 8 * j, t, n_tile * p.BN);
               if (++b_slot == p.b_slots) { b_slot = 0; b_phase ^= 1; }
             }
           }
@@ -186,281 +123,105 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (one elected thread, whole loop)
-    if (elect_one()) {
-      const uint32_t idesc = make_idesc_bf16(128, p.BN, 0, 0);
-      const uint64_t a_tmpl = make_smem_desc(0, 16, kHaloW * 128, 2);
-      const uint64_t b_tmpl = make_smem_desc(0, 16, 1024, 2);
-      const uint32_t a0 = smem_u32(a_base) >> 4, b0 = smem_u32(b_base) >> 4;
-      const uint32_t btile16 = (uint32_t)p.b_tile_bytes >> 4;
-      const int last = p.cchunks - 1;
-      int a_slot = 0, b_slot = 0;
-      uint32_t a_phase = 0, b_phase = 0;
-      int it = 0;
-      if (p.resident) { mbar_wait(&b_full[0], 0); tc_fence_after(); }
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-        const int as = it & 1;
-        mbar_wait(&tempty[as], ((it >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * p.acc_stride;
-        for (int cc = 0; cc <= last; ++cc) {
-          mbar_wait(&a_full[a_slot], a_phase);
-          tc_fence_after();
-          DBG_TS(1, it);
-          const uint64_t ad = a_tmpl + (uint64_t)(a0 + (uint32_t)a_slot * (kASlotBytes >> 4));
-          const int ks = (cc == last) ? p.ksteps_last : 4;
-          const uint32_t acc_first = cc != 0 ? 1u : 0u;
-          if (p.resident) {
-            const uint64_t bd = b_tmpl + (uint64_t)(b0 + (uint32_t)(cc * 9) * btile16);
-            switch (ks) {
-              case 4: halo_issue9<4>(d_tmem, ad, bd, btile16, idesc, acc_first); break;
-              case 3: halo_issue9<3>(d_tmem, ad, bd, btile16, idesc, acc_first); break;
-              case 2: halo_issue9<2>(d_tmem, ad, bd, btile16, idesc, acc_first); break;
-              default: halo_issue9<1>(d_tmem, ad, bd, btile16, idesc, acc_first); break;
-            }
-          } else {
-#pragma unroll
-            for (int t = 0; t < 9; ++t) {
-              const int kh = t / 3, kw = t - kh * 3;
-              mbar_wait(&b_full[b_slot], b_phase);
-              tc_fence_after();
-              const uint64_t at = ad + (uint64_t)((kh * kHaloW + kw) * 8);
-              const uint64_t bd = b_tmpl + (uint64_t)(b0 + (uint32_t)b_slot * btile16);
-#pragma unroll
-              for (int k = 0; k < 4; ++k)
-                if (k < ks) umma_f16(d_tmem, at + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), idesc, (t | k) ? 1u : acc_first);
-              umma_commit(&b_empty[b_slot]);
-              if (++b_slot == p.b_slots) { b_slot = 0; b_phase ^= 1; }
-            }
+  } else {
+    // ------------------------------------------------------------------ consumers: MMA + epilogue
+    const uint32_t g = warp >> 2;               // warpgroup: tile rows 8g .. 8g + 7
+    const bool leader = (threadIdx.x & 127) == 0;
+    float* my_stats = s_stats + (size_t)warp * 2 * p.cout_pad;
+    const uint64_t a_tmpl = make_smem_desc(0, kPlane, kHaloW * 16, 0);
+    const uint64_t b_tmpl = make_smem_desc(0, p.BN * 16, 128, 0);
+    const uint32_t a0 = smem_u32(a_base) + g * 8 * kHaloW * 16, b0 = smem_u32(b_base);
+    const uint32_t b64 = (64 * 16) >> 4;                  // 64 weight rows of 16 bytes
+    const uint32_t bk16 = (uint32_t)(2 * p.BN * 16) >> 4;  // next K = 16 step: two channel-group planes
+    const uint32_t ak16 = (2 * kPlane) >> 4;
+    const int nb16 = p.BN >> 4;
+    const int last = p.cchunks - 1;
+    ConvEpi e{y, p.has_bias ? bias : nullptr, addend, p.y_ld, p.addend_ld, 0, p.Cout, p.emit_stats, p.cout_pad};
+    float acc[NB * 8];
+    int a_slot = 0, b_slot = 0;
+    uint32_t a_phase = 0, b_phase = 0;
+    if (p.resident) mbar_wait(&b_full[0], 0);
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      PendingRelease pend;
+      for (int cc = 0; cc <= last; ++cc) {
+        mbar_wait(&a_full[a_slot], a_phase);
+        const uint64_t ad = a_tmpl + (uint64_t)((a0 + (uint32_t)a_slot * kASlotBytes) >> 4);
+        const int ks = (cc == last) ? p.ksteps_last : 4;
+        if (p.resident) {
+          wgmma_fence();
+          for (int t = 0; t < 9; ++t) {
+            const int kh = t / 3, kw = t - kh * 3;
+            const uint64_t at = ad + (uint64_t)(kh * kHaloW + kw);     // (kh*10 + kw) pixels of 16 B
+            const uint64_t bt = b_tmpl + (uint64_t)((b0 + (uint32_t)(cc * 9 + t) * (uint32_t)p.b_tile_bytes) >> 4);
+            for (int k = 0; k < ks; ++k)
+              wgmma_row<NB, 0, 0>(acc, nb16, at + (uint64_t)(k * ak16), bt + (uint64_t)(k * bk16), b64, (cc | t | k) != 0);
           }
-          umma_commit(&a_empty[a_slot]);
-          if (cc == last) umma_commit(&tfull[as]);
-          DBG_TS(2, it);
-          if (++a_slot == p.a_slots) { a_slot = 0; a_phase ^= 1; }
-        }
-      }
-      pdl_launch_late();    // every MMA of this CTA is issued: only the last epilogue and the statistics remain
-    }
-    __syncwarp();
-  } else if (warp >= 4) {
-    // ------------------------------------------------------------------ epilogue (thread == output pixel)
-    const uint32_t ew = warp - 4;
-    const uint32_t q = ew & 3;                  // TMEM lane quarter == warp % 4
-    const uint32_t half = ew >> 2;              // which half of the accumulator columns
-    const int m = q * 32 + lane;
-    const int th = m >> 3, tw = m & 7;
-    float* my_stats = s_stats + (size_t)q * 2 * p.cout_pad;
-    const int nchunks = p.BN >> 4;
-    const int ch_begin = half ? (nchunks + 1) / 2 : 0;
-    const int ch_end = half ? nchunks : (nchunks + 1) / 2;
-    int it = 0;
-    if constexpr (FAST) {
-      // n_tiles == 1, BN <= 64: this warp owns 16-column groups {2*half, 2*half+1} of its 32 pixels
-      float acc1[2][16], acc2[2][16];
-#pragma unroll
-      for (int k = 0; k < 2; ++k)
-#pragma unroll
-        for (int j = 0; j < 16; ++j) { acc1[k][j] = 0.f; acc2[k][j] = 0.f; }
-      const bool issuer = (warp == 4) && (lane == 0);
-      const uint32_t sw = (uint32_t)m & 7u;
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-        const int as = it & 1;
-        const int tw_i = tile % p.tiles_w;
-        const int th_i = (tile / p.tiles_w) % p.tiles_h;
-        const int img = tile / (p.tiles_w * p.tiles_h);
-        const int ho = th_i * kTH + th, wo = tw_i * kTW + tw;
-        const bool valid = (ho < p.H) && (wo < p.W);
-        const size_t pix = ((size_t)img * p.H + ho) * p.W + wo;
-        uint8_t* srow = stage_base + (size_t)as * kStageTile + (size_t)m * 128;
-        mbar_wait(&tfull[as], (it >> 1) & 1);
-        tc_fence_after();
-        if (warp == 4 && lane == 0) DBG_TS(3, it);
-        const uint32_t taddr = tmem_base + ((q * 32u) << 16) + as * p.acc_stride;
-#pragma unroll
-        for (int k = 0; k < 2; ++k) {
-          const int c0 = ((int)half * 2 + k) * 16;
-          if (c0 < p.BN) {                        // warp-uniform
-            uint32_t r[16];
-            tmem_ld16(taddr + c0, r);
-            tmem_ld_wait();
-            float v[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
-            if (p.has_bias) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) v[j] += (c0 + j < p.Cout) ? __ldg(bias + c0 + j) : 0.f;
-            }
-            if (addend != nullptr && valid && c0 + 16 <= p.Cout) {
-              const __nv_bfloat16* ap = addend + pix * p.addend_ld + c0;
-              float a0[8], a1[8];
-              load8(ap, a0);
-              load8(ap + 8, a1);
-#pragma unroll
-              for (int j = 0; j < 8; ++j) { v[j] += a0[j]; v[8 + j] += a1[j]; }
-            }
-            uint32_t pk[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) pk[j] = pack_bf16x2(v[2 * j], v[2 * j + 1]);
-            const uint32_t lc = (uint32_t)c0 >> 3;               // logical 16-byte chunk inside the 128-byte pixel row
-            st_shared_v4(srow + ((lc ^ sw) << 4), pk[0], pk[1], pk[2], pk[3]);
-            st_shared_v4(srow + (((lc + 1) ^ sw) << 4), pk[4], pk[5], pk[6], pk[7]);
-            if (p.emit_stats && valid) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const float lo = bf16_lo(pk[j]), hi = bf16_hi(pk[j]);
-                acc1[k][2 * j] += lo;          acc1[k][2 * j + 1] += hi;
-                acc2[k][2 * j] += lo * lo;     acc2[k][2 * j + 1] += hi * hi;
-              }
-            }
+          wgmma_commit();
+          wgmma_wait<1>();
+          pend.release(leader);
+          pend.bar0 = &a_empty[a_slot];
+        } else {
+          for (int t = 0; t < 9; ++t) {
+            const int kh = t / 3, kw = t - kh * 3;
+            mbar_wait(&b_full[b_slot], b_phase);
+            const uint64_t at = ad + (uint64_t)(kh * kHaloW + kw);
+            const uint64_t bt = b_tmpl + (uint64_t)((b0 + (uint32_t)b_slot * (uint32_t)p.b_tile_bytes) >> 4);
+            wgmma_fence();
+            for (int k = 0; k < ks; ++k)
+              wgmma_row<NB, 0, 0>(acc, nb16, at + (uint64_t)(k * ak16), bt + (uint64_t)(k * bk16), b64, (cc | t | k) != 0);
+            wgmma_commit();
+            wgmma_wait<1>();
+            pend.release(leader);
+            pend.bar0 = &b_empty[b_slot];
+            if (t == 8) pend.bar1 = &a_empty[a_slot];
+            if (++b_slot == p.b_slots) { b_slot = 0; b_phase ^= 1; }
           }
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty[as]);       // the accumulator buffer is free: the next tile's MMAs may start
-        fence_proxy_async();                            // my st.shared -> visible to the TMA (async proxy)
-        if (issuer) tma_store_wait_read<0>();           // the previous tile's store has drained the OTHER staging buffer
-        named_barrier_sync(1, 256);
-        if (issuer) {
-          tma_store_4d(&tmY, stage_base + (size_t)as * kStageTile, 0, tw_i * kTW, th_i * kTH, img);
-          tma_store_commit();
-          DBG_TS(4, it);
-        }
+        if (++a_slot == p.a_slots) { a_slot = 0; a_phase ^= 1; }
       }
-      if (issuer) tma_store_wait_all<0>();
-      if (p.emit_stats) {
-#pragma unroll
-        for (int k = 0; k < 2; ++k) {
-          const int c0 = ((int)half * 2 + k) * 16;
-          if (c0 < p.BN) {
-            h_butterfly16(acc1[k], lane);
-            h_butterfly16(acc2[k], lane);
-            if (lane < 16) {
-              my_stats[c0 + lane] += acc1[k][0];
-              my_stats[p.cout_pad + c0 + lane] += acc2[k][0];
-            }
-          }
-        }
-      }
-    } else
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-      const int as = it & 1;
+      wgmma_wait<0>();
+      pend.release(leader);
+      if (tile + (int)gridDim.x >= p.total_tiles && g == 0 && (threadIdx.x & 127) == 0)
+        pdl_launch_late();    // every MMA of this CTA is done: only the last epilogue and the statistics remain
+
       const int m_tile = tile / p.n_tiles, n_tile = tile - m_tile * p.n_tiles;
       const int tw_i = m_tile % p.tiles_w;
       const int th_i = (m_tile / p.tiles_w) % p.tiles_h;
       const int img = m_tile / (p.tiles_w * p.tiles_h);
-      const int ho = th_i * kTH + th, wo = tw_i * kTW + tw;
-      const bool valid = (ho < p.H) && (wo < p.W);
-      const int n0 = n_tile * p.BN;
-      const size_t pix = ((size_t)img * p.H + ho) * p.W + wo;
-      mbar_wait(&tfull[as], (it >> 1) & 1);
-      tc_fence_after();
-      if (warp == 4 && lane == 0) DBG_TS(3, it);
-      const uint32_t taddr = tmem_base + ((q * 32u) << 16) + as * p.acc_stride;
-
-      // one 16-column group: bias, gradient addend, bf16 store, batch statistics of the stored values
-      auto epi16 = [&](const uint32_t* r, int c0) {
-        float v[16];
+      bool valid[2];
+      size_t pix[2];
 #pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
-        if (p.has_bias) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] += (c0 + j < p.Cout) ? __ldg(bias + c0 + j) : 0.f;
-        }
-        const bool affine = fold.accum == nullptr && fold.scale != nullptr;   // evaluation: BN folded into the epilogue
-        if (affine) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-            if (c0 + j < p.Cout) v[j] = v[j] * __ldg(fold.scale + c0 + j) + __ldg(fold.shift + c0 + j);
-        }
-        if (addend != nullptr && valid && c0 + 16 <= p.Cout) {
-          const __nv_bfloat16* ap = addend + pix * p.addend_ld + c0;
-          float a0[8], a1[8];
-          load8(ap, a0);
-          load8(ap + 8, a1);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) { v[j] += a0[j]; v[8 + j] += a1[j]; }
-        }
-        if (affine && fold.relu) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
-        }
-        uint32_t pk[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) pk[j] = pack_bf16x2(v[2 * j], v[2 * j + 1]);
-        if (valid) {
-          __nv_bfloat16* dst = y + pix * p.y_ld + c0;
-          if (c0 + 16 <= p.Cout) {
-            uint4* d4 = reinterpret_cast<uint4*>(dst);
-            d4[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-            d4[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              if (c0 + j < p.Cout) dst[j] = __float2bfloat16_rn(v[j]);
-          }
-        }
-        if (p.emit_stats) {
-          float s1[16], s2[16];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float lo = valid ? bf16_lo(pk[j]) : 0.f, hi = valid ? bf16_hi(pk[j]) : 0.f;
-            s1[2 * j] = lo;      s1[2 * j + 1] = hi;
-            s2[2 * j] = lo * lo; s2[2 * j + 1] = hi * hi;
-          }
-          h_butterfly16(s1, lane);
-          h_butterfly16(s2, lane);
-          if (lane < 16) {
-            my_stats[c0 + lane] += s1[0];
-            my_stats[p.cout_pad + c0 + lane] += s2[0];
-          }
-        }
-      };
-
-      int ch = ch_begin;
-      for (; ch + 2 <= ch_end; ch += 2) {
-        if (n0 + ch * 16 >= p.Cout) break;      // warp-uniform
-        uint32_t r[32];
-        tmem_ld32(taddr + ch * 16, r);
-        tmem_ld_wait();
-        if (warp == 4 && lane == 0) DBG_TS(5, it);
-        epi16(r, n0 + ch * 16);
-        if (n0 + ch * 16 + 16 < p.Cout) epi16(r + 16, n0 + ch * 16 + 16);
+      for (int r = 0; r < 2; ++r) {
+        const int m = (int)(g * 64 + (warp & 3) * 16 + (lane >> 2)) + 8 * r;   // accumulator row == pixel of the tile
+        const int ho = th_i * kTH + (m >> 3), wo = tw_i * kTW + (m & 7);
+        valid[r] = (ho < p.H) && (wo < p.W);
+        pix[r] = ((size_t)img * p.H + ho) * p.W + wo;
       }
-      if (ch < ch_end && n0 + ch * 16 < p.Cout) {
-        uint32_t r[16];
-        tmem_ld16(taddr + ch * 16, r);
-        tmem_ld_wait();
-        epi16(r, n0 + ch * 16);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[as]);
-      if (warp == 4 && lane == 0) DBG_TS(4, it);
+      conv_epilogue<NB>(acc, nb16, n_tile * p.BN, valid, pix, e, fold, my_stats, lane);
     }
   }
-  if (threadIdx.x == 0) DBG_TS(6, 1);
 
-  tc_fence_before();
   __syncthreads();
   if (p.emit_stats) {
     if (fold.accum != nullptr) {
-      bn_fold_tail(fold, s_stats, p.cout_pad, tmem_ptr_smem + 1);          // statistics finalised by the last CTA of this launch
+      bn_fold_tail(fold, s_stats, p.cout_pad, ticket);          // statistics finalised by the last CTA of this launch
     } else {
       float* out = stats_partials + (size_t)blockIdx.x * 2 * p.cout_pad;
-      for (int i = threadIdx.x; i < 2 * p.cout_pad; i += kHThreads)
-        out[i] = (s_stats[i] + s_stats[2 * p.cout_pad + i]) + (s_stats[4 * p.cout_pad + i] + s_stats[6 * p.cout_pad + i]);
+      for (int i = threadIdx.x; i < 2 * p.cout_pad; i += kHThreads) {
+        float v = 0.f;
+        for (int s = 0; s < kStatSlots; ++s) v += s_stats[2 * s * p.cout_pad + i];
+        out[i] = v;
+      }
     }
   }
-  if (warp == 2) { tc_fence_after(); tmem_dealloc(tmem_base, p.tmem_cols); }
 }
 
 // Cout tile width: minimise (waves x per-tile clocks) with per-tile clocks = max(tensor issue, L2->smem fill).
 // A narrow tile costs ~32 clocks per MMA regardless of N (the A operand read from shared memory bounds it).
-// Two CTAs may share an SM when their Cout tile needs at most 128 accumulator columns per buffer (2 x 128 of the 512 TMEM
-// columns), 80 registers x 384 threads and half of the shared memory: CTAs of DIFFERENT launches (the 0.5x and 1.0x
+// Two CTAs may share an SM when their Cout tile needs at most 128 accumulator columns (64 registers per consumer thread)
+// and half of the shared memory: CTAs of DIFFERENT launches (the 0.5x and 1.0x
 // passes, the HRNet branch streams, a PDL successor's prologue) then overlap their fill/drain latencies on one SM, and a
-// 256-tile layer runs as one round of 296 slots instead of two rounds of 148. B200SEG_CORESIDENT=0 restores one CTA/SM.
+// 256-tile layer runs as one round of 264 slots instead of two rounds of 132. B200SEG_CORESIDENT=0 restores one CTA/SM.
 static bool halo_coresident_enabled() {
   static const bool on = []() { const char* e = getenv("B200SEG_CORESIDENT"); return !(e && e[0] == '0'); }();
   return on;
@@ -469,13 +230,11 @@ constexpr size_t kHalfSmBudget = 115712;   // (228 KB - 2 x 1 KB reserved) / 2
 
 // Shared-memory layout of a CTA for a given Cout tile: returns the CTAs per SM it allows (2, 1, or 0 = does not fit).
 struct HaloSmem { int resident, a_slots, b_slots; size_t bytes; };
-static int halo_smem_layout(int BN, int n_tiles, int cchunks, int cout_pad, HaloSmem& L, int stage_bytes = 0) {
+static int halo_smem_layout(int BN, int n_tiles, int cchunks, int cout_pad, HaloSmem& L) {
   const size_t b_tile = (size_t)(BN * 128 + 1023) / 1024 * 1024;
-  const size_t fixed = 1024 + (2 * kMaxASlots + 2 * kMaxBSlots2 + 4) * 8 + 16 + (size_t)4 * 2 * cout_pad * 4 +
-                       (size_t)stage_bytes;
+  const size_t fixed = 1024 + (2 * kMaxASlots + 2 * kMaxBSlots2) * 8 + 16 + (size_t)kStatSlots * 2 * cout_pad * 4;
   const size_t resident_bytes = (size_t)9 * cchunks * b_tile;
-  // the staged epilogue (stage_bytes != 0) is built for one CTA per SM only
-  for (int occ = (halo_coresident_enabled() && BN <= 128 && stage_bytes == 0) ? 2 : 1; occ >= 1; --occ) {
+  for (int occ = (halo_coresident_enabled() && BN <= 128) ? 2 : 1; occ >= 1; --occ) {
     const size_t budget = (occ == 2 ? kHalfSmBudget : (size_t)227 * 1024) - fixed - (size_t)smem_reserve() / occ;
     if (n_tiles == 1 && resident_bytes + 2 * (size_t)kASlotBytes <= budget) {
       const int as_ = (int)((budget - resident_bytes) / kASlotBytes);
@@ -536,18 +295,8 @@ static int halo_plan(int n, int h, int w, int cin, int cout, HaloParams& p, size
   p.cout_pad = (cout + 15) / 16 * 16;
   p.total_tiles = m_tiles * p.n_tiles;
   p.b_tile_bytes = (p.BN * 128 + 1023) / 1024 * 1024;
-  p.acc_stride = p.BN <= 32 ? 32 : (p.BN <= 64 ? 64 : (p.BN <= 128 ? 128 : 256));
-  p.tmem_cols = 2 * p.acc_stride;
-  // staged TMA-store epilogue with register-resident statistics for the narrow (HBM-bound) layers (opt-in).
-  // Measured (round 2, whole step): the staged epilogue is faster per launch but needs the full register file, i.e. one
-  // CTA per SM, and the 48 / 64-channel layers it applies to gain more from two co-resident CTAs per SM (39.4 vs
-  // 40.3 ms per step) - it is therefore OFF unless B200SEG_HALO_FAST=1.
-  static const bool fast_enabled = []() { const char* e = getenv("B200SEG_HALO_FAST"); return e && e[0] == '1'; }();
-  const bool fast = fast_enabled && p.n_tiles == 1 && p.BN <= 64;
-  p.stage_bytes = fast ? 2 * kStageTile : 0;
-  { const char* e = getenv("B200SEG_DBG"); p.dbg = e ? atoi(e) : 0; }
   HaloSmem L;
-  occ = halo_smem_layout(p.BN, p.n_tiles, p.cchunks, p.cout_pad, L, p.stage_bytes);
+  occ = halo_smem_layout(p.BN, p.n_tiles, p.cchunks, p.cout_pad, L);
   if (occ >= 1) { p.resident = L.resident; p.a_slots = L.a_slots; p.b_slots = L.b_slots; smem_bytes = L.bytes; }
   if (occ < 1) return B200SEG_E_BADARG;
   // one CTA per SM unless the co-resident configuration was chosen (occupancy is bounded by shared memory and registers)
@@ -557,14 +306,15 @@ static int halo_plan(int n, int h, int w, int cin, int cout, HaloParams& p, size
   return 0;
 }
 
-// {kernel 1 = halo, BN, n_tiles, grid, smem bytes, ring depth (A slots), CTAs per SM, TMEM columns, resident weights, B slots}
+// {kernel 1 = halo, BN, n_tiles, grid, smem bytes, ring depth (A slots), CTAs per SM, accumulator registers per consumer
+// thread, resident weights, B slots}
 int conv3x3_halo_plan_info(int n, int h, int w, int cin, int cout, int32_t* out) {
   HaloParams p;
   size_t smem_bytes;
   int grid, occ;
   if (int rc = halo_plan(n, h, w, cin, cout, p, smem_bytes, grid, occ)) return rc;
   out[0] = 1; out[1] = p.BN; out[2] = p.n_tiles; out[3] = grid; out[4] = (int32_t)smem_bytes; out[5] = p.a_slots;
-  out[6] = occ; out[7] = p.tmem_cols; out[8] = p.resident; out[9] = p.b_slots;
+  out[6] = occ; out[7] = p.BN / 2; out[8] = p.resident; out[9] = p.b_slots;
   return 0;
 }
 
@@ -591,51 +341,37 @@ int conv3x3_halo_launch(int n, int h, int w, int cin, int in_ld, const void* in,
   if ((reinterpret_cast<uintptr_t>(in) & 15) || (reinterpret_cast<uintptr_t>(wts) & 15) ||
       (reinterpret_cast<uintptr_t>(out) & 15) || (reinterpret_cast<uintptr_t>(addend) & 15) || (addend && addend_ld % 8))
     return B200SEG_E_BADARG;
-  CUtensorMap tmA, tmB, tmY;
-  {
+  CUtensorMap tmA, tmB;
+  {   // one box = one 8-channel plane of the halo tile
     uint64_t dims[4] = {(uint64_t)cin, (uint64_t)w, (uint64_t)h, (uint64_t)n};
     uint64_t strides[3] = {(uint64_t)in_ld * 2, (uint64_t)w * in_ld * 2, (uint64_t)h * w * in_ld * 2};
-    uint32_t box[4] = {64, (uint32_t)kHaloW, (uint32_t)kHaloH, 1};
-    int rc = encode_bf16(&tmA, in, 4, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_128B);
+    uint32_t box[4] = {8, (uint32_t)kHaloW, (uint32_t)kHaloH, 1};
+    int rc = encode_bf16(&tmA, in, 4, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_NONE);
     if (rc) return rc;
   }
-  if (p.stage_bytes) {   // output tile: 64 channels x 8 x 16 pixels, clipped to [cout, w, h] by the tensor map
-    uint64_t dims[4] = {(uint64_t)cout, (uint64_t)w, (uint64_t)h, (uint64_t)n};
-    uint64_t strides[3] = {(uint64_t)out_ld * 2, (uint64_t)w * out_ld * 2, (uint64_t)h * w * out_ld * 2};
-    uint32_t box[4] = {64, (uint32_t)kTW, (uint32_t)kTH, 1};
-    int rc = encode_bf16(&tmY, out, 4, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (rc) return rc;
-  } else {
-    tmY = tmA;   // unused
-  }
-  {
+  {   // one box = one 8-channel plane (BN rows x 16 bytes) of one tap
     uint64_t dims[3] = {(uint64_t)cin, 9, (uint64_t)cout};
     uint64_t strides[2] = {(uint64_t)cin * 2, (uint64_t)9 * cin * 2};
-    uint32_t box[3] = {64, 1, (uint32_t)p.BN};
-    int rc = encode_bf16(&tmB, wts, 3, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_128B);
+    uint32_t box[3] = {8, 1, (uint32_t)p.BN};
+    int rc = encode_bf16(&tmB, wts, 3, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_NONE);
     if (rc) return rc;
   }
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv3x3_halo_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(conv3x3_halo_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) return (int)e;
-    e = cudaFuncSetAttribute(conv3x3_halo_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e != cudaSuccess) return (int)e;
-    e = cudaFuncSetAttribute(conv3x3_halo_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHalfSmBudget);
+    e = cudaFuncSetAttribute(conv3x3_halo_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHalfSmBudget);
     if (e != cudaSuccess) return (int)e;
     // two CTAs per SM need (almost) the whole 228 KB as shared memory: ask for the maximum carve-out explicitly
-    e = cudaFuncSetAttribute(conv3x3_halo_kernel<2, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    e = cudaFuncSetAttribute(conv3x3_halo_kernel<2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     if (e != cudaSuccess) return (int)e;
     attr_set = true;
   }
-  if (affine && p.stage_bytes) return B200SEG_E_BADARG;   // the staged epilogue (opt-in, training) has no affine mode
   cudaError_t e =
-      p.stage_bytes ? launch_k(conv3x3_halo_kernel<1, true>, dim3(grid), dim3(kHThreads), smem_bytes, stream, tmA, tmB, tmY, p,
-                               (__nv_bfloat16*)out, bias, stats_partials, (const __nv_bfloat16*)addend, fd)
-      : occ == 2    ? launch_k(conv3x3_halo_kernel<2, false>, dim3(grid), dim3(kHThreads), smem_bytes, stream, tmA, tmB, tmY, p,
-                               (__nv_bfloat16*)out, bias, stats_partials, (const __nv_bfloat16*)addend, fd)
-                    : launch_k(conv3x3_halo_kernel<1, false>, dim3(grid), dim3(kHThreads), smem_bytes, stream, tmA, tmB, tmY, p,
-                               (__nv_bfloat16*)out, bias, stats_partials, (const __nv_bfloat16*)addend, fd);
+      occ == 2 ? launch_k(conv3x3_halo_kernel<2>, dim3(grid), dim3(kHThreads), smem_bytes, stream, tmA, tmB, p,
+                          (__nv_bfloat16*)out, bias, stats_partials, (const __nv_bfloat16*)addend, fd)
+               : launch_k(conv3x3_halo_kernel<1>, dim3(grid), dim3(kHThreads), smem_bytes, stream, tmA, tmB, p,
+                          (__nv_bfloat16*)out, bias, stats_partials, (const __nv_bfloat16*)addend, fd);
   return e == cudaSuccess ? 0 : (int)e;
 }
 
@@ -645,12 +381,12 @@ int conv3x3_halo_launch(int n, int h, int w, int cin, int in_ld, const void* in,
 int conv_igemm_occupancy(int occ_variant, int smem_bytes);
 int conv3x3_halo_occupancy(int occ_variant, int smem_bytes) {
   int nb = -1;
-  cudaFuncSetAttribute(conv3x3_halo_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(conv3x3_halo_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHalfSmBudget);
-  cudaFuncSetAttribute(conv3x3_halo_kernel<2, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  cudaFuncSetAttribute(conv3x3_halo_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  cudaFuncSetAttribute(conv3x3_halo_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHalfSmBudget);
+  cudaFuncSetAttribute(conv3x3_halo_kernel<2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   cudaError_t e = occ_variant == 2
-      ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, conv3x3_halo_kernel<2, false>, kHThreads, (size_t)smem_bytes)
-      : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, conv3x3_halo_kernel<1, false>, kHThreads, (size_t)smem_bytes);
+      ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, conv3x3_halo_kernel<2>, kHThreads, (size_t)smem_bytes)
+      : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, conv3x3_halo_kernel<1>, kHThreads, (size_t)smem_bytes);
   return e == cudaSuccess ? nb : -(int)e;
 }
 
@@ -682,8 +418,8 @@ extern "C" void b200seg_debug_occupancy_report(void) {
          pr.regsPerBlock, pr.sharedMemPerMultiprocessor, pr.sharedMemPerBlockOptin, pr.reservedSharedMemPerBlock,
          pr.maxBlocksPerMultiProcessor, pr.maxThreadsPerMultiProcessor);
   b200seg::conv3x3_halo_occupancy(2, 1024);     // sets the attributes of both builds
-  b200seg::occupancy_report_one("conv3x3_halo_kernel<2>", b200seg::conv3x3_halo_kernel<2, false>, b200seg::kHThreads);
-  b200seg::occupancy_report_one("conv3x3_halo_kernel<1>", b200seg::conv3x3_halo_kernel<1, false>, b200seg::kHThreads);
+  b200seg::occupancy_report_one("conv3x3_halo_kernel<2>", b200seg::conv3x3_halo_kernel<2>, b200seg::kHThreads);
+  b200seg::occupancy_report_one("conv3x3_halo_kernel<1>", b200seg::conv3x3_halo_kernel<1>, b200seg::kHThreads);
   b200seg::conv_igemm_occupancy_report();
   fflush(stdout);
 }

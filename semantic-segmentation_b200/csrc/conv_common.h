@@ -9,7 +9,7 @@ struct ConvPlan {
   int BN, n_tiles, cout_pad;
   int TH, TW, tiles_h, tiles_w, total_tiles, grid;
   int a_bytes, b_bytes, stage_bytes, nstages;
-  int acc_stride, tmem_cols, occ;
+  int acc_regs, occ;     // fp32 accumulator registers per consumer thread (BN / 2), CTAs per SM
   size_t smem_bytes;
 };
 int conv_plan(const b200seg_conv_desc* d, ConvPlan* pl);
@@ -18,16 +18,16 @@ int conv_plan(const b200seg_conv_desc* d, ConvPlan* pl);
 int smem_reserve();
 
 // Launch-width tuning, read once from the environment (defaults: see tune() in conv_igemm.cu). The two-scale step keeps
-// 8+ independent kernel chains in flight and is bound by SM occupancy, not by the latency of any chain: the sum over its
-// launches of (duration x share of the SMs held) equals the step time (profiles/r2_sm_time.txt) while the launch /
-// dependency floor of the captured program is 4 ms (B200SEG_DRY). A launch that spreads a small layer over every SM pays
-// its per-CTA fixed cost (prologue, pipeline fill, drain) 148-296 times; these knobs give every CTA a minimum amount of
+// 8+ independent kernel chains in flight, so SM occupancy rather than the latency of one chain bounds it (B200SEG_DRY
+// replays the captured program with empty kernels to show its launch / dependency floor). A launch that spreads a small
+// layer over every SM pays
+// its per-CTA fixed cost (prologue, pipeline fill, drain) once per SM or twice; these knobs give every CTA a minimum amount of
 // work instead, so narrow launches of different streams run side by side.
 struct Tune {
   int conv_min_clk;      // B200SEG_CONV_MIN_CLK: modelled tensor clocks of work per convolution CTA (0: widest grid)
   int wgrad_min_clk;     // B200SEG_WGRAD_MIN_CLK: the same per weight-gradient work unit (bounds the pixel splits)
   int ew_items;          // B200SEG_EW_ITEMS: 16-byte items per thread of the element-wise BatchNorm passes
-  int ew_ctas_per_sm;    // B200SEG_EW_CTAS_PER_SM: grid cap of those passes (x 148)
+  int ew_ctas_per_sm;    // B200SEG_EW_CTAS_PER_SM: grid cap of those passes (x SMs)
   int red_items;         // B200SEG_RED_ITEMS: pixel rows per thread of bn_bwd_reduce
   int red_ctas_per_sm;   // B200SEG_RED_CTAS_PER_SM
   int rs_items;          // B200SEG_RS_ITEMS: items per thread of the resample / fuse / accumulate passes

@@ -1,19 +1,14 @@
-// Implicit-GEMM convolution for sm_100a.
+// Implicit-GEMM convolution for sm_90a.
 //
 //   GEMM view:  D[pixels, cout] = sum over (tap, cin-chunk) A[pixels, chunk] * B[cout, chunk]^T
 //   A operand:  NHWC activations fetched by 4-D tiled TMA boxes (chunk x TW x TH x 1). A filter tap is a shifted
 //               box; out-of-image coordinates are zero-filled by the TMA unit, which *is* the im2col padding.
 //               Stride-2 convolutions use the tensor map's element strides.
 //   B operand:  bf16 weights [cout][tap][cin] through a 3-D map (chunk x 1 x BN).
-//   MMA:        tcgen05.mma cta_group::1 kind::f16, M = 128 pixels (TH x TW patch), N = BN <= 256, K = 16 per
-//               instruction, fp32 accumulators double-buffered in TMEM (2 x 256 columns).
-//   Epilogue:   4 warps, thread == pixel: tcgen05.ld -> (+bias) -> round to bf16 -> 16-byte stores; per-channel
-//               sum / sum-of-squares of the *stored* values for training-mode BatchNorm (network/mynn.py:18-24)
-//               reduced with a shuffle butterfly and kept per-warp in shared memory (deterministic order).
-//   Schedule:   persistent CTAs (<= 1 per SM), static round-robin tile order, warp-specialised (384 threads):
-//               warp 0 TMA producer (one elected lane), warp 1 MMA issuer (one elected thread runs the whole loop:
-//               barrier waits + unrolled tcgen05.mma issue), warp 2 TMEM allocator, warps 4-11 epilogue (two warps
-//               per TMEM lane quarter, half of the accumulator columns each).
+//   MMA:        wgmma, M = 128 pixels (TH x TW patch) split over two consumer warpgroups of 64 rows, N = BN <= 256,
+//               K = 16 per instruction, fp32 accumulators in registers.
+//   Epilogue:   conv_epi.cuh, from the registers; BatchNorm sums of the *stored* values kept per warp (fixed order).
+//   Schedule:   persistent CTAs, round-robin tiles; 288 threads: warps 0-7 consumers, warp 8 TMA producer.
 //   Launch:     programmatic dependent launch (launch.h): the prologue overlaps the previous kernel's tail.
 #include <cstdio>
 #include <cstring>
@@ -24,7 +19,7 @@
 #include "../../include/b200seg.h"
 #include "conv_common.h"
 #include "bn_fold.cuh"
-#include "vec.cuh"
+#include "conv_epi.cuh"
 
 namespace b200seg {
 
@@ -40,73 +35,47 @@ struct ConvKParams {
   int y_ld, out_fp32, has_bias, emit_stats, cout_pad, addend_ld;
   int layout_type, sbo;
   int a_bytes, b_bytes, stage_bytes, nstages;
-  int acc_stride, tmem_cols;    // two TMEM accumulator buffers of acc_stride = pow2 >= BN columns
 };
 
-constexpr int kThreads = 384;
+constexpr int kThreads = 288;
 constexpr int kMaxStages = 8;
 constexpr size_t kHalfSmBudget = 115712;   // (228 KB - 2 x 1 KB reserved) / 2: two CTAs per SM (see conv3x3_halo.cu)
 
-// Sum v[0..15] over the 32 lanes of the warp: afterwards v[0] holds the total for channel (lane & 15).
-__device__ __forceinline__ void butterfly16(float (&v)[16], uint32_t lane) {
-#pragma unroll
-  for (int off = 8; off >= 1; off >>= 1) {
-    const bool up = (lane & off) != 0;
-#pragma unroll
-    for (int i = 0; i < off; ++i) {
-      const float send = up ? v[i] : v[i + off];
-      const float keep = up ? v[i + off] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-    }
-  }
-  v[0] += __shfl_xor_sync(0xffffffffu, v[0], 16);
-}
-
-template <int OCC>     // CTAs per SM the register budget allows (2: co-resident narrow tiles)
+// OCC: CTAs per SM; the two-per-SM build holds at most 128 accumulator columns (64 registers per consumer thread).
+template <int OCC>
 __global__ void __launch_bounds__(kThreads, OCC)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const ConvKParams p, void* __restrict__ y, const float* __restrict__ bias,
                   float* __restrict__ stats_partials, const __nv_bfloat16* __restrict__ addend, const BnFoldDev fold) {
+  constexpr int NB = OCC == 2 ? 8 : 16;    // 16-column accumulator blocks
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [stages][A|B] (1024-aligned) | barriers | tmem ptr | stats[4][2][cout_pad]
+  // carve: [stages][A|B] (1024-aligned) | barriers | ticket | stats[kStatSlots][2][cout_pad]
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* stage_base = smem;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)p.nstages * p.stage_bytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kMaxStages;
-  uint64_t* tfull_bar = bars + 2 * kMaxStages;
-  uint64_t* tempty_bar = bars + 2 * kMaxStages + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * kMaxStages + 4);
-  float* s_stats = reinterpret_cast<float*>(tmem_ptr_smem + 4);   // [4 warps][2][cout_pad]
+  uint32_t* ticket = reinterpret_cast<uint32_t*>(bars + 2 * kMaxStages);
+  float* s_stats = reinterpret_cast<float*>(ticket + 4);
 
   const uint32_t warp = threadIdx.x >> 5;
   const uint32_t lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < p.nstages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tfull_bar[s], 1); mbar_init(&tempty_bar[s], 8); }
+    for (int s = 0; s < p.nstages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_ptr_smem, p.tmem_cols);
-    tmem_relinquish();
-  }
   if (p.emit_stats) {
-    for (int i = threadIdx.x; i < 4 * 2 * p.cout_pad; i += kThreads) s_stats[i] = 0.f;
+    for (int i = threadIdx.x; i < kStatSlots * 2 * p.cout_pad; i += kThreads) s_stats[i] = 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   pdl_sync();   // the prologue above overlapped the previous kernel; global memory is touched only below
 
   const int kblocks = p.ntaps * p.cchunks;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ------------------------------------------------------------------ TMA producer (one elected lane)
     if (elect_one()) {
       int stage = 0;
@@ -132,169 +101,74 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (one elected thread, whole loop)
-    if (elect_one()) {
-      const uint32_t idesc = make_idesc_bf16(128, p.BN, 0, 0);
-      const uint64_t tmpl = make_smem_desc(0, 16, p.sbo, p.layout_type);
-      const uint32_t s0 = smem_u32(stage_base) >> 4, stage16 = (uint32_t)p.stage_bytes >> 4, a16 = (uint32_t)p.a_bytes >> 4;
-      const int ksteps = p.KC >> 4;
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-        const int as = it & 1;
-        mbar_wait(&tempty_bar[as], ((it >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * p.acc_stride;
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint64_t adesc = tmpl + (uint64_t)(s0 + (uint32_t)stage * stage16);
-          const uint64_t bdesc = adesc + (uint64_t)a16;
-          // advancing K by 16 bf16 = 32 bytes inside the swizzle atom: +2 in the 16-byte-unit address field
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            if (k < ksteps) umma_f16(d_tmem, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc, (kb | k) != 0);
-          umma_commit(&empty_bar[stage]);
-          if (kb == kblocks - 1) umma_commit(&tfull_bar[as]);
-          if (++stage == p.nstages) { stage = 0; phase ^= 1; }
-        }
+  } else {
+    // ------------------------------------------------------------------ consumers: MMA + epilogue
+    const uint32_t g = warp >> 2;              // warpgroup: pixel rows 64g .. 64g + 63 of the tile
+    const bool leader = (threadIdx.x & 127) == 0;
+    float* my_stats = s_stats + (size_t)warp * 2 * p.cout_pad;
+    const uint64_t tmpl = make_smem_desc(0, 16, p.sbo, p.layout_type);
+    const uint32_t s0 = smem_u32(stage_base);
+    const uint32_t a_off = g * (uint32_t)(p.a_bytes / 2);
+    const uint32_t b64 = (uint32_t)(64 * p.KC * 2) >> 4;
+    const int ksteps = p.KC >> 4;
+    const int nb16 = p.BN >> 4;
+    ConvEpi e{y, p.has_bias ? bias : nullptr, addend, p.y_ld, p.addend_ld, p.out_fp32, p.Cout, p.emit_stats, p.cout_pad};
+    float acc[NB * 8];
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      PendingRelease pend;
+      for (int kb = 0; kb < kblocks; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = s0 + (uint32_t)stage * (uint32_t)p.stage_bytes;
+        const uint64_t adesc = tmpl + (uint64_t)((sa + a_off) >> 4);
+        const uint64_t bdesc = tmpl + (uint64_t)((sa + (uint32_t)p.a_bytes) >> 4);
+        wgmma_fence();
+        // advancing K by 16 bf16 = 32 bytes inside the swizzle atom: +2 in the 16-byte-unit address field
+        for (int k = 0; k < ksteps; ++k)
+          wgmma_row<NB, 0, 0>(acc, nb16, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), b64, (kb | k) != 0);
+        wgmma_commit();
+        wgmma_wait<1>();
+        pend.release(leader);
+        pend.bar0 = &empty_bar[stage];
+        if (++stage == p.nstages) { stage = 0; phase ^= 1; }
       }
-      pdl_launch_late();    // every MMA of this CTA is issued: only the last epilogue and the statistics remain
-    }
-    __syncwarp();
-  } else if (warp >= 4) {
-    // ------------------------------------------------------------------ epilogue
-    const uint32_t ew = warp - 4;
-    const uint32_t q = ew & 3;                 // TMEM sub-partition == warp % 4
-    const uint32_t half = ew >> 2;             // which half of the accumulator columns
-    const int m = q * 32 + lane;               // accumulator row == pixel within the tile
-    const int th = m / p.TW, tw = m - th * p.TW;
-    float* my_stats = s_stats + (size_t)q * 2 * p.cout_pad;
-    const int nchunks = p.BN >> 4;
-    const int ch_begin = half ? (nchunks + 1) / 2 : 0;
-    const int ch_end = half ? nchunks : (nchunks + 1) / 2;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-      const int as = it & 1;
+      wgmma_wait<0>();
+      pend.release(leader);
+      if (tile + (int)gridDim.x >= p.total_tiles && g == 0 && (threadIdx.x & 127) == 0)
+        pdl_launch_late();    // every MMA of this CTA is done: only the last epilogue and the statistics remain
+
       const int m_tile = tile / p.n_tiles, n_tile = tile - m_tile * p.n_tiles;
       const int tw_i = m_tile % p.tiles_w;
       const int th_i = (m_tile / p.tiles_w) % p.tiles_h;
       const int img = m_tile / (p.tiles_w * p.tiles_h);
-      const int hs = th_i * p.TH + th, ws = tw_i * p.TW + tw;
-      const bool valid = (hs < p.sub_H) && (ws < p.sub_W);
-      const int ho = hs * p.out_stride + p.out_off_h, wo = ws * p.out_stride + p.out_off_w;
-      const int n0 = n_tile * p.BN;
-      const size_t pix = ((size_t)img * p.Ho + ho) * p.Wo + wo;
-
-      mbar_wait(&tfull_bar[as], (it >> 1) & 1);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((q * 32u) << 16) + as * p.acc_stride;
-
-      auto epi16 = [&](const uint32_t* r, int c0) {
-        float v[16];
+      bool valid[2];
+      size_t pix[2];
 #pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
-        if (p.has_bias) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] += (c0 + j < p.Cout) ? __ldg(bias + c0 + j) : 0.f;
-        }
-        const bool affine = fold.accum == nullptr && fold.scale != nullptr;   // evaluation: BN folded into the epilogue
-        if (affine) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-            if (c0 + j < p.Cout) v[j] = v[j] * __ldg(fold.scale + c0 + j) + __ldg(fold.shift + c0 + j);
-        }
-        if (addend != nullptr && valid && c0 + 16 <= p.Cout) {
-          const __nv_bfloat16* ap = addend + pix * p.addend_ld + c0;
-          float a0[8], a1[8];
-          load8(ap, a0);
-          load8(ap + 8, a1);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) { v[j] += a0[j]; v[8 + j] += a1[j]; }
-        }
-        if (affine && fold.relu) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
-        }
-        if (p.out_fp32) {
-          if (valid) {
-            float* dst = reinterpret_cast<float*>(y) + pix * p.y_ld + c0;
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              if (c0 + j < p.Cout) dst[j] = v[j];
-          }
-          return;
-        }
-        uint32_t pk[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) pk[j] = pack_bf16x2(v[2 * j], v[2 * j + 1]);
-        if (valid) {
-          __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(y) + pix * p.y_ld + c0;
-          if (c0 + 16 <= p.Cout) {
-            uint4* d4 = reinterpret_cast<uint4*>(dst);
-            d4[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-            d4[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              if (c0 + j < p.Cout) dst[j] = __float2bfloat16_rn(v[j]);
-          }
-        }
-        if (p.emit_stats) {
-          float s1[16], s2[16];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float lo = valid ? bf16_lo(pk[j]) : 0.f, hi = valid ? bf16_hi(pk[j]) : 0.f;
-            s1[2 * j] = lo;      s1[2 * j + 1] = hi;
-            s2[2 * j] = lo * lo; s2[2 * j + 1] = hi * hi;
-          }
-          butterfly16(s1, lane);
-          butterfly16(s2, lane);
-          if (lane < 16) {
-            my_stats[c0 + lane] += s1[0];
-            my_stats[p.cout_pad + c0 + lane] += s2[0];
-          }
-        }
-      };
-
-      int ch = ch_begin;
-      for (; ch + 2 <= ch_end; ch += 2) {
-        if (n0 + ch * 16 >= p.Cout) break;     // warp-uniform
-        uint32_t r[32];
-        tmem_ld32(taddr + ch * 16, r);
-        tmem_ld_wait();
-        epi16(r, n0 + ch * 16);
-        if (n0 + ch * 16 + 16 < p.Cout) epi16(r + 16, n0 + ch * 16 + 16);
+      for (int r = 0; r < 2; ++r) {
+        const int m = (int)(g * 64 + (warp & 3) * 16 + (lane >> 2)) + 8 * r;   // accumulator row == pixel of the tile
+        const int th = m / p.TW, tw = m - th * p.TW;
+        const int hs = th_i * p.TH + th, ws = tw_i * p.TW + tw;
+        valid[r] = (hs < p.sub_H) && (ws < p.sub_W);
+        const int ho = hs * p.out_stride + p.out_off_h, wo = ws * p.out_stride + p.out_off_w;
+        pix[r] = ((size_t)img * p.Ho + ho) * p.Wo + wo;
       }
-      if (ch < ch_end && n0 + ch * 16 < p.Cout) {
-        uint32_t r[16];
-        tmem_ld16(taddr + ch * 16, r);
-        tmem_ld_wait();
-        epi16(r, n0 + ch * 16);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[as]);
+      conv_epilogue<NB>(acc, nb16, n_tile * p.BN, valid, pix, e, fold, my_stats, lane);
     }
   }
 
-  tc_fence_before();
   __syncthreads();
   if (p.emit_stats) {
     if (fold.accum != nullptr) {
-      bn_fold_tail(fold, s_stats, p.cout_pad, tmem_ptr_smem + 1);          // statistics finalised by the last CTA of this launch
+      bn_fold_tail(fold, s_stats, p.cout_pad, ticket);          // statistics finalised by the last CTA of this launch
     } else {
       float* out = stats_partials + (size_t)blockIdx.x * 2 * p.cout_pad;
       for (int i = threadIdx.x; i < 2 * p.cout_pad; i += kThreads) {
-        out[i] = (s_stats[i] + s_stats[2 * p.cout_pad + i]) + (s_stats[4 * p.cout_pad + i] + s_stats[6 * p.cout_pad + i]);
+        float v = 0.f;
+        for (int s = 0; s < kStatSlots; ++s) v += s_stats[2 * s * p.cout_pad + i];
+        out[i] = v;
       }
     }
-  }
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, p.tmem_cols);
   }
 }
 
@@ -361,11 +235,11 @@ static int plan_geom(const LaunchGeom& g, ConvPlan* pl) {
   pl->a_bytes = 128 * KC * 2;
   pl->b_bytes = pl->BN * KC * 2;
   pl->stage_bytes = (pl->a_bytes + pl->b_bytes + 1023) / 1024 * 1024;
-  pl->acc_stride = pl->BN <= 32 ? 32 : (pl->BN <= 64 ? 64 : (pl->BN <= 128 ? 128 : 256));
-  pl->tmem_cols = 2 * pl->acc_stride;
-  size_t fixed = 1024 /*align slack*/ + (2 * kMaxStages + 4) * 8 + 16 + (size_t)4 * 2 * pl->cout_pad * 4;
-  // two CTAs per SM for narrow Cout tiles (TMEM 2 x <=128 columns, 80 registers, half of the shared memory each), so that
-  // CTAs of different launches overlap their fill / drain latencies on one SM; else one CTA with the deepest ring
+  pl->acc_regs = pl->BN / 2;
+  size_t fixed = 1024 /*align slack*/ + 2 * kMaxStages * 8 + 16 + (size_t)kStatSlots * 2 * pl->cout_pad * 4;
+  // two CTAs per SM for narrow Cout tiles (<= 128 accumulator columns = 64 registers per consumer thread, half of the
+  // shared memory each), so that CTAs of different launches overlap their fill / drain latencies on one SM; else one CTA
+  // with the deepest ring
   int occ = (coresident_enabled() && pl->BN <= 128) ? 2 : 1;
   int nst = 0;
   for (; occ >= 1; --occ) {
@@ -515,10 +389,9 @@ static int launch_geom(const LaunchGeom& g, const void* a, const void* w, const 
   p.TH = pl.TH; p.TW = pl.TW; p.tiles_h = pl.tiles_h; p.tiles_w = pl.tiles_w; p.total_tiles = pl.total_tiles;
   p.y_ld = g.out_ld; p.out_fp32 = g.out_fp32; p.has_bias = g.has_bias; p.emit_stats = g.emit_stats;
   p.cout_pad = pl.cout_pad; p.addend_ld = addend_ld;
-  p.layout_type = pl.KC == 64 ? 2 : (pl.KC == 32 ? 4 : 6);
+  p.layout_type = pl.KC == 64 ? 1 : (pl.KC == 32 ? 2 : 3);   // 128B / 64B / 32B swizzle
   p.sbo = 8 * pl.KC * 2;
   p.a_bytes = pl.a_bytes; p.b_bytes = pl.b_bytes; p.stage_bytes = pl.stage_bytes; p.nstages = pl.nstages;
-  p.acc_stride = pl.acc_stride; p.tmem_cols = pl.tmem_cols;
 
   static bool attr_set = false;
   if (!attr_set) {
@@ -577,12 +450,12 @@ using namespace b200seg;
 extern "C" size_t b200seg_conv2d_stats_elems(const b200seg_conv_desc* d) {
   ConvPlan pl;
   if (conv_plan(d, &pl) != 0) return 0;
-  return (size_t)B200SEG_MAX_GRID * 2 * ((d->cout + 15) / 16 * 16);   // [grid <= 296][2][roundup16(cout)]
+  return (size_t)B200SEG_MAX_GRID * 2 * ((d->cout + 15) / 16 * 16);   // [grid <= B200SEG_MAX_GRID][2][roundup16(cout)]
 }
 
 // Host-only: the launch plan of a forward (which = 0) or stride-1 data-gradient (which = 1) convolution, for tests and
 // tuning scripts. out[10] = {kernel (1 halo / 0 per-tap), BN, n_tiles, grid, dynamic smem bytes, ring depth, CTAs per SM,
-// TMEM columns, resident weights (halo), weight slots (halo)}.
+// accumulator registers per consumer thread, resident weights (halo), weight slots (halo)}.
 extern "C" int b200seg_conv2d_plan_info(const b200seg_conv_desc* d, int32_t which, int32_t* out) {
   if (!desc_ok(d) || !out || which < 0 || which > 1) return B200SEG_E_BADARG;
   if (which == 1 && d->stride != 1) return B200SEG_E_BADARG;
@@ -598,7 +471,7 @@ extern "C" int b200seg_conv2d_plan_info(const b200seg_conv_desc* d, int32_t whic
   ConvPlan pl;
   if (int rc = plan_geom(g, &pl)) return rc;
   out[0] = 0; out[1] = pl.BN; out[2] = pl.n_tiles; out[3] = pl.grid; out[4] = (int32_t)pl.smem_bytes; out[5] = pl.nstages;
-  out[6] = pl.occ; out[7] = pl.tmem_cols; out[8] = 0; out[9] = 0;
+  out[6] = pl.occ; out[7] = pl.acc_regs; out[8] = 0; out[9] = 0;
   return 0;
 }
 

@@ -79,7 +79,7 @@ blend_kernel(const float* __restrict__ a, const float* __restrict__ x, const flo
 
 static inline int egrid(long long total) {
   long long b = (total + 255) / 256;
-  const long long cap = 148LL * 16;
+  const long long cap = (long long)B200SEG_MAX_CTAS * 16;
   return (int)(b < 1 ? 1 : (b > cap ? cap : b));
 }
 

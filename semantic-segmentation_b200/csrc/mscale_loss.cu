@@ -465,7 +465,7 @@ lo_bwd_kernel(const MsGeom g, const float* __restrict__ D, const float* __restri
 
 static inline int blocks_for(long long total, int threads) {
   long long b = (total + threads - 1) / threads;
-  const long long cap = 148LL * 16;
+  const long long cap = (long long)B200SEG_MAX_CTAS * 16;
   return (int)(b < 1 ? 1 : (b > cap ? cap : b));
 }
 

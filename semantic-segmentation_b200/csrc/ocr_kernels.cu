@@ -1,7 +1,7 @@
 // Small-K softmax glue around the OCR (object-contextual representation) GEMMs.
 //
 // The two skinny products of SpatialGather (network/ocr_utils.py:34-46) and ObjectAttentionBlock
-// (network/ocr_utils.py:95-119) run on the tcgen05 convolution / weight-gradient kernels with the 19 classes padded to
+// (network/ocr_utils.py:95-119) run on the tensor-core convolution / weight-gradient kernels with the 19 classes padded to
 // a 32-wide bf16 operand; what remains here are the softmaxes between them (K = num_classes <= 32):
 //   spatial softmax  : over the H*W pixels of each (image, class) map  -> probs bf16 [pixels][32]
 //   class softmax    : over the classes of each pixel, with the key_channels^-0.5 scale -> sim bf16 [pixels][32]
@@ -272,23 +272,23 @@ __global__ void cast_rows_kernel(const float* __restrict__ src, int src_ld, __nv
 }
 
 
-// db[c] += sum_rows dy[row][c]  for c < C  (conv bias gradient of the logit heads; dy bf16 [rows][ld])
-__global__ void __launch_bounds__(256)
+// db[c] += sum_rows dy[row][c]  for c < C  (conv bias gradient of the logit heads; dy bf16 [rows][ld]).
+// One CTA in a fixed summation order, so the gradient is the same bit for bit in every run (a few MB per call).
+constexpr int kColsumLanes = 32;   // row lanes; x 32 columns = 1024 threads
+__global__ void __launch_bounds__(1024)
 colsum_kernel(const __nv_bfloat16* __restrict__ dy, int ld, long long rows, int C, float* __restrict__ db) {
   pdl_sync();
-  // thread (r, c): 8 row-lanes x 32 columns
   const int c = threadIdx.x & 31, r = threadIdx.x >> 5;
   float acc = 0.f;
   if (c < C)
-    for (long long row = (long long)blockIdx.x * 8 + r; row < rows; row += (long long)gridDim.x * 8)
-      acc += __bfloat162float(dy[row * ld + c]);
-  __shared__ float s[8][32];
+    for (long long row = r; row < rows; row += kColsumLanes) acc += __bfloat162float(dy[row * ld + c]);
+  __shared__ float s[kColsumLanes][32];
   s[r][c] = acc;
   __syncthreads();
   if (r == 0 && c < C) {
     float t = 0.f;
-    for (int i = 0; i < 8; ++i) t += s[i][c];
-    atomicAdd(db + c, t);
+    for (int i = 0; i < kColsumLanes; ++i) t += s[i][c];
+    db[c] += t;
   }
 }
 
@@ -304,7 +304,7 @@ using namespace b200seg;
 
 static inline int pix_blocks(long long P) {
   long long b = (P + 255) / 256;
-  return (int)(b < 1 ? 1 : (b > 296 ? 296 : b));
+  return (int)(b < 1 ? 1 : (b > B200SEG_MAX_GRID ? B200SEG_MAX_GRID : b));
 }
 
 extern "C" int32_t b200seg_spatial_softmax_blocks(int32_t P) { return pix_blocks(P); }
@@ -360,7 +360,7 @@ extern "C" int b200seg_cast_rows(const float* src, int32_t src_ld, void* dst_bf1
   if (!src || !dst_bf16) return B200SEG_E_BADARG;
   long long total = rows * C;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > B200SEG_MAX_CTAS * 8) blocks = B200SEG_MAX_CTAS * 8;
   launch_k(cast_rows_kernel, dim3(blocks), dim3(256), 0, (cudaStream_t)stream, src, src_ld, (__nv_bfloat16*)dst_bf16,
            dst_ld, rows, C, accumulate);
   RET_LAUNCH();
@@ -368,9 +368,7 @@ extern "C" int b200seg_cast_rows(const float* src, int32_t src_ld, void* dst_bf1
 
 extern "C" int b200seg_bias_grad(const void* dy_bf16, int32_t ld, int64_t rows, int32_t C, float* db, void* stream) {
   if (!dy_bf16 || !db || C > 32) return B200SEG_E_BADARG;
-  long long b = (rows + 7) / 8;
-  if (b > 148 * 4) b = 148 * 4;
-  launch_k(colsum_kernel, dim3((int)b), dim3(256), 0, (cudaStream_t)stream, (const __nv_bfloat16*)dy_bf16, ld, rows,
+  launch_k(colsum_kernel, dim3(1), dim3(kColsumLanes * 32), 0, (cudaStream_t)stream, (const __nv_bfloat16*)dy_bf16, ld, rows,
            C, db);
   RET_LAUNCH();
 }

@@ -69,7 +69,7 @@ extern "C" int b200seg_pack_weights(const b200seg_pack_item* items, const int32_
 }
 
 extern "C" int b200seg_abi_version(void) { return 1; }
-extern "C" const char* b200seg_build_info(void) { return "b200seg sm_100a " __DATE__ " " __TIME__; }
+extern "C" const char* b200seg_build_info(void) { return "b200seg sm_90a " __DATE__ " " __TIME__; }
 
 extern "C" int b200seg_pack_weight(const float* w_oihw, int32_t o, int32_t i, int32_t ksize, void* w_ohwi,
                                    void* w_dgrad, int32_t o_pad, void* stream) {
@@ -77,7 +77,7 @@ extern "C" int b200seg_pack_weight(const float* w_oihw, int32_t o, int32_t i, in
   if (!w_oihw || o <= 0 || i <= 0 || (ksize != 1 && ksize != 3)) return B200SEG_E_BADARG;
   const size_t total = (size_t)o * i * ksize * ksize;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > B200SEG_MAX_CTAS * 8) blocks = B200SEG_MAX_CTAS * 8;
   launch_k(pack_weight_kernel, dim3(blocks), dim3(256), 0, (cudaStream_t)stream, w_oihw, o, i, ksize,
            (__nv_bfloat16*)w_ohwi, (__nv_bfloat16*)w_dgrad, o_pad);
   cudaError_t e = cudaGetLastError();

@@ -17,7 +17,7 @@ namespace b200seg {
 
 static inline int pool_grid(long long total_threads) {
   long long b = (total_threads + 255) / 256;
-  const long long cap = 148LL * 8;
+  const long long cap = (long long)B200SEG_MAX_CTAS * 8;
   return (int)(b < cap ? (b > 0 ? b : 1) : cap);
 }
 

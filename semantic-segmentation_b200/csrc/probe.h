@@ -5,24 +5,10 @@
 #ifdef __cplusplus
 extern "C" {
 #endif
-typedef struct b200seg_probe_operand {
-  int32_t rows, cols;            /* global bf16 matrix [rows][cols], cols contiguous */
-  int32_t box_cols, box_rows;    /* TMA box */
-  int32_t nboxes, c0, r0, dcol, drow, smem_stride;
-  int32_t swizzle_bytes;         /* 0, 32, 64, 128 */
-} b200seg_probe_operand;
-typedef struct b200seg_probe_desc {
-  b200seg_probe_operand a, b;
-  int32_t M, N, ksteps;
-  int32_t a_off, a_lbo, a_sbo, a_layout, a_base, a_major, a_kstep;
-  int32_t b_off, b_lbo, b_sbo, b_layout, b_base, b_major, b_kstep;
-} b200seg_probe_desc;
 /* Slow, obviously-correct CUDA-core direct convolution with the numerics contract of b200seg_conv2d_fwd (bf16 operands,
  * fp32 accumulate, one rounding): the on-device cross-check of the GPU op tests. */
 int b200seg_conv2d_fwd_direct(const b200seg_conv_desc* d, const void* x, const void* w_ohwi, const float* bias,
                               void* y, void* stream);
-/* tcgen05 shared-memory descriptor probe (profiles/r1_umma_probe.txt) */
-int b200seg_umma_probe(const b200seg_probe_desc* p, const void* A, const void* B, float* D, void* stream);
 #ifdef __cplusplus
 }
 #endif

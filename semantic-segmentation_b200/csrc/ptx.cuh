@@ -1,4 +1,4 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc/mma/commit/ld).
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma.
 // Everything here is hand-written against the PTX ISA for CUDA 12.9; no CUTLASS/CuTe dependency.
 #pragma once
 #include <cstdint>
@@ -67,13 +67,12 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t phase) {
 // Every kernel of the library is launched with the programmatic-stream-serialization attribute (launch.h) and runs
 //   <prologue that touches no global data>; pdl_wait(); <main work>; pdl_launch_late(); <tail>
 // pdl_wait blocks until the preceding grid on the stream has completed and flushed its writes; pdl_launch lets the next
-// grid on the stream start its own prologue (barrier init, TMEM allocation, descriptor prefetch) under this grid's body.
+// grid on the stream start its own prologue (barrier init, descriptor prefetch) under this grid's body.
 // Because *every* kernel executes pdl_wait before it completes, completion is transitive along the stream.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-// Late trigger (default; -DB200SEG_PDL_EARLY builds the variant that triggers at the start of every kernel; measured 37.95
-// vs 38.24 ms on the two-scale step, profiles/r2_ab_switches.txt): a dependent grid that becomes resident at the START
-// of its predecessor holds registers, shared memory and TMEM on the SMs for the predecessor's whole duration while it
+// Late trigger (default; -DB200SEG_PDL_EARLY builds the variant that triggers at the start of every kernel): a dependent grid that becomes resident at the START
+// of its predecessor holds registers and shared memory on the SMs for the predecessor's whole duration while it
 // sits in griddepcontrol.wait - on a step bound by what fits on the SMs that residency is paid by the other streams. The
 // default therefore triggers the dependent when a CTA has finished its main loop (pdl_launch_late), so only the successor's
 // prologue overlaps the predecessor's tail; kernels without an explicit late trigger fall back to the implicit one at exit.
@@ -134,78 +133,68 @@ __device__ __forceinline__ void st_shared_v4(void* dst, uint32_t a, uint32_t b, 
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(smem_u32(dst)), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// ---------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
+// D[64 x N] (+)= A[64 x 16] * B[16 x N]^T: bf16 smem operands, fp32 register accumulators. Thread (warp w, lane l) holds,
+// per 8-column chunk c, d[4c + {0,1}] = row 16w + l/4, columns 8c + 2(l%4) + {0,1}, and d[4c + {2,3}] = row + 8: so
+// narrow MMAs over consecutive column blocks fill the registers a wide one would. TA / TB: 0 K-major, 1 MN-major.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 covers bf16/fp16 inputs with fp32 accumulate.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB));
 }
-// Arrive on an mbarrier once every previously issued tcgen05.mma of this thread has completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 16 consecutive 32-bit columns: thread t of the warp gets lane (taddr.lane + t), columns col..col+15.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n32(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n48(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %26, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, %27, %28;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n64(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB));
+}
 
-// Shared-memory matrix descriptor (sm_100 "version 1"). layout_type: 0 none, 2 = 128B, 4 = 64B, 6 = 32B swizzle.
-// lbo/sbo are byte offsets (multiples of 16).
+// Shared-memory matrix descriptor (sm_90). layout_type: 0 = no swizzle (8 x 16 B core matrices), 1 = 128B, 2 = 64B,
+// 3 = 32B swizzle. lbo/sbo are byte offsets (multiples of 16). K-major: SBO = stride between 8-row groups (M / N),
+// LBO = stride between the two core matrices of a K = 16 step (no swizzle only). MN-major swizzled: LBO = stride
+// between swizzle atoms along M / N, SBO = stride between 8-row groups along K.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                   uint32_t layout_type, uint32_t base_offset = 0) {
+                                                   uint32_t layout_type) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;                       // descriptor version for sm_100
-  d |= static_cast<uint64_t>(base_offset & 7) << 49;
-  d |= static_cast<uint64_t>(layout_type & 7) << 61;
+  d |= static_cast<uint64_t>(layout_type & 3) << 62;
   return d;
-}
-// Instruction descriptor for kind::f16: bf16 x bf16 -> fp32, M x N tile, majors: 0 = K-major, 1 = MN-major.
-__host__ __device__ __forceinline__ uint32_t make_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_mn_major,
-                                                             uint32_t b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) |
-         ((M >> 4) << 24);
 }
 
 // 16-byte fp32 reduction into global memory (sm_90+): fire-and-forget, no return value, no latency chain.

@@ -201,7 +201,7 @@ image_prep_kernel(const float* __restrict__ img, int N, int H, int W, __nv_bfloa
 static inline int ew_grid(long long total_threads) {
   const long long per = 256LL * (tune().rs_items > 0 ? tune().rs_items : 1);
   long long b = (total_threads + per - 1) / per;
-  const long long cap = 148LL * 8;
+  const long long cap = (long long)B200SEG_MAX_CTAS * 8;
   return (int)(b < cap ? (b > 0 ? b : 1) : cap);
 }
 

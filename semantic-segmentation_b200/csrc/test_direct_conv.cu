@@ -1,5 +1,5 @@
 // TEST LIBRARY (libb200seg_test.so, not the product): a CUDA-core direct convolution with the same numerics contract as
-// the tcgen05 path (bf16 operands, fp32 accumulate, one final rounding), the on-device cross-check of tests/test_gpu_ops.py.
+// the wgmma path (bf16 operands, fp32 accumulate, one final rounding), the on-device cross-check of tests/test_gpu_ops.py.
 #include "ptx.cuh"
 #include "launch.h"
 #include "../../include/b200seg.h"
@@ -48,7 +48,7 @@ extern "C" int b200seg_conv2d_fwd_direct(const b200seg_conv_desc* d, const void*
   const int Wo = (d->w + 2 * d->pad - d->ksize) / d->stride + 1;
   const size_t total = (size_t)d->n * Ho * Wo * d->cout;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > B200SEG_MAX_CTAS * 16) blocks = B200SEG_MAX_CTAS * 16;
   launch_k(direct_conv_kernel, dim3(blocks), dim3(256), 0, (cudaStream_t)stream, (const __nv_bfloat16*)x,
            (const __nv_bfloat16*)w_ohwi, d->has_bias ? bias : nullptr, y, d->n, d->h, d->w, d->cin, d->cout, d->ksize,
            d->stride, d->pad, Ho, Wo, d->x_ld, d->y_ld, d->out_fp32);

@@ -1,16 +1,17 @@
-// Weight-gradient convolution as a tcgen05 GEMM with both operands MN-major (pixels are the reduction dimension):
+// Weight-gradient convolution as a wgmma GEMM with both operands MN-major (pixels are the reduction dimension):
 //
 //   dW[co][ci][kh][kw] += sum_{n,ho,wo} dy[n,ho,wo,co] * x[n, ho*s+kh-p, wo*s+kw-p, ci]
 //
-//   A = dy  [pixels][cout]  -> M = 128 output channels (two 64-channel SWIZZLE_128B blocks of 128 pixel-rows)
+//   A = dy  [pixels][cout]  -> M = 128 output channels (two 64-channel SWIZZLE_128B blocks of 128 pixel-rows), one
+//                              block per consumer warpgroup
 //   B = x   [pixels][cin]   -> N <= 256 input channels (64-channel blocks), one shifted TMA box per filter tap
-//   D[tap]  = fp32 accumulator in TMEM, taps of a group side by side (taps_in_group * N <= 512 columns)
+//   D[tap]  = fp32 accumulators in registers, taps of a group side by side (taps_in_group * N <= 256 columns)
 //
 // Work unit = (M tile, N tile, tap group, pixel split). Units are distributed round-robin over a persistent grid; each
-// unit reduces its share of the pixels in TMEM. The gradient accumulator is fp32 in the kernels' own [Cout][tap][Cin]
+// unit reduces its share of the pixels in registers. The gradient accumulator is fp32 in the kernels' [Cout][tap][Cin]
 // ("OHWI") layout, so an accumulator row is a contiguous run of input channels:
 //   * splits == 1 (low-resolution / wide layers: enough (tile, tap-group) items to fill the SMs): exactly one unit owns
-//     every gradient element, which it adds with 16-byte red.global.add.v4.f32 — no workspace, no second kernel,
+//     every gradient element, which it adds with fire-and-forget reductions — no workspace, no second kernel,
 //     deterministic;
 //   * splits  > 1 (high-resolution narrow layers): units store fp32 slabs and wgrad_reduce_kernel sums the splits in a
 //     fixed order (deterministic) with coalesced float4 traffic.
@@ -21,6 +22,7 @@
 #include "tma_host.h"
 #include "launch.h"
 #include "conv_common.h"
+#include "conv_epi.cuh"
 #include "../../include/b200seg.h"
 
 namespace b200seg {
@@ -31,23 +33,30 @@ struct WgradParams {
   int TH, TW, tiles_h, tiles_w, pix_tiles;
   int m_tiles, n_tiles, tap_groups, taps_per_group, splits, total_units;
   int nblocksB_max;
-  int halo;              // 3x3 stride-1: one x halo tile per pixel tile, taps are row-shifted descriptors
-  int ntile_w;           // N tile width in channels (256, or 128 in halo mode)
-  int b_block_bytes;     // bytes of one 64-channel B block (16384 dense, 24576 halo)
-  int unit_n;            // accumulator row pitch of a unit slab (= min(256, Cin))
+  int ntile_w;           // N tile width in channels (64, 128 or 256)
+  int unit_n;            // accumulator row pitch of a unit slab (= min(ntile_w, Cin))
   long long unit_stride; // floats per unit slab
   int a_slot_bytes, b_slot_bytes, b_slots;
   int direct;            // splits == 1: units add straight into the gradient accumulator
-  int tmem_cols;         // TMEM allocation: 512, or a power of two <= 256 in the co-resident configuration
 };
 
-constexpr int kWThreads = 256;
+constexpr int kWThreads = 288;       // warps 0-7: two consumer warpgroups, warp 8: TMA producer
 constexpr int kABlock = 128 * 128;   // 128 pixel rows x 64 channels bf16
 constexpr int kMaxBSlots = 6;
+constexpr int kWAccCols = 256;       // accumulator columns per consumer thread row (128 registers)
+
+// one MN-major MMA of width 16 * w (w <= 4 blocks: inside one 64-channel swizzle atom)
+__device__ __forceinline__ void wgmma_mn(float* d, int w, uint64_t a, uint64_t b, uint32_t scale_d) {
+  if (w >= 4) wgmma_n64<1, 1>(d, a, b, scale_d);
+  else if (w == 3) wgmma_n48<1, 1>(d, a, b, scale_d);
+  else if (w == 2) wgmma_n32<1, 1>(d, a, b, scale_d);
+  else wgmma_n16<1, 1>(d, a, b, scale_d);
+}
 
 __global__ void __launch_bounds__(kWThreads, 1)
 wgrad_igemm_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constant__ CUtensorMap tmX,
                    const WgradParams p, float* __restrict__ ws, float* __restrict__ dw) {
+  constexpr int NB = kWAccCols / 16;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* a_base = smem;                               // 2 slots
@@ -57,24 +66,16 @@ wgrad_igemm_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_consta
   uint64_t* a_empty = bars + 2;         // [2]
   uint64_t* b_full = bars + 4;          // [kMaxBSlots]
   uint64_t* b_empty = bars + 4 + kMaxBSlots;
-  uint64_t* acc_full = bars + 4 + 2 * kMaxBSlots;
-  uint64_t* acc_empty = acc_full + 1;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(acc_empty + 1);
 
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) { tma_prefetch_desc(&tmDy); tma_prefetch_desc(&tmX); }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < 2; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 1); }
-    for (int s = 0; s < p.b_slots; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 1); }
-    mbar_init(acc_full, 1);
-    mbar_init(acc_empty, 4);
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&tmDy);
+    tma_prefetch_desc(&tmX);
+    for (int s = 0; s < 2; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 2); }
+    for (int s = 0; s < p.b_slots; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 2); }
     fence_barrier_init();
   }
-  if (warp == 2) { tmem_alloc(tmem_ptr_smem, p.tmem_cols); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   pdl_sync();   // the prologue above overlapped the previous kernel; global memory is touched only below
 
   // unit decode helpers (identical in every role)
@@ -86,7 +87,7 @@ wgrad_igemm_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_consta
     m_tile = item / p.n_tiles;
   };
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (elect_one()) {   // one elected lane runs the whole producer loop (TMA operands stay in uniform registers)
       int a_slot = 0, b_slot = 0;
       uint32_t a_phase = 0, b_phase = 0;
@@ -108,16 +109,6 @@ wgrad_igemm_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_consta
           if (a_two)
             tma_load_4d(&tmDy, &a_full[a_slot], sa + kABlock, m_tile * 128 + 64, tw_i * p.TW, th_i * p.TH, img);
           if (++a_slot == 2) { a_slot = 0; a_phase ^= 1; }
-          if (p.halo) {
-            mbar_wait(&b_empty[b_slot], b_phase ^ 1);
-            uint8_t* sb = b_base + (size_t)b_slot * p.b_slot_bytes;
-            mbar_arrive_expect_tx(&b_full[b_slot], nblk * 18 * 10 * 128);
-            for (int b = 0; b < nblk; ++b)
-              tma_load_4d(&tmX, &b_full[b_slot], sb + (size_t)b * p.b_block_bytes, n0 + b * 64, tw_i * p.TW - 1,
-                          th_i * p.TH - 1, img);
-            if (++b_slot == p.b_slots) { b_slot = 0; b_phase ^= 1; }
-            continue;
-          }
           for (int tap = tap0; tap < tap1; ++tap) {
             const int kh = tap / p.ksize, kw = tap - kh * p.ksize;
             mbar_wait(&b_empty[b_slot], b_phase ^ 1);
@@ -133,118 +124,89 @@ wgrad_igemm_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_consta
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (elect_one()) {   // one elected thread: barrier waits + unrolled tcgen05.mma issue for the whole CTA
-      // 16 pixels per MMA = two 8-pixel tile rows: dy rows are dense (2048 B per K step); halo x rows sit 10 apart
-      const uint64_t a_tmpl = make_smem_desc(0, kABlock, 1024, 2);
-      const uint64_t bh_tmpl = make_smem_desc(0, p.b_block_bytes, 1280, 2);
-      const uint64_t bd_tmpl = make_smem_desc(0, kABlock, 1024, 2);
-      const uint32_t a0 = smem_u32(a_base) >> 4, b0 = smem_u32(b_base) >> 4;
-      const uint32_t aslot16 = (uint32_t)p.a_slot_bytes >> 4, bslot16 = (uint32_t)p.b_slot_bytes >> 4;
-      int a_slot = 0, b_slot = 0;
-      uint32_t a_phase = 0, b_phase = 0;
-      int uit = 0;
-      for (int unit = blockIdx.x; unit < p.total_units; unit += gridDim.x, ++uit) {
-        int m_tile, n_tile, tg, split;
-        decode(unit, m_tile, n_tile, tg, split);
-        const int n0 = n_tile * p.ntile_w;
-        const int Nn = min(p.ntile_w, p.Cin - n0);         // multiple of 16
-        const uint32_t idesc = make_idesc_bf16(128, Nn, 1, 1);
-        const int tap0 = tg * p.taps_per_group, tap1 = min(p.taps, tap0 + p.taps_per_group);
-        mbar_wait(acc_empty, (uit & 1) ^ 1);
-        tc_fence_after();
-        uint32_t acc = 0;
-        for (int t = split; t < p.pix_tiles; t += p.splits) {
-          mbar_wait(&a_full[a_slot], a_phase);
-          tc_fence_after();
-          const uint64_t ad = a_tmpl + (uint64_t)(a0 + (uint32_t)a_slot * aslot16);
-          if (p.halo) {
-            mbar_wait(&b_full[b_slot], b_phase);
-            tc_fence_after();
-            const uint64_t bd = bh_tmpl + (uint64_t)(b0 + (uint32_t)b_slot * bslot16);
-            uint32_t d_tmem = tmem_base;
-            for (int tap = tap0; tap < tap1; ++tap, d_tmem += Nn) {
-              const int kh = tap / 3, kw = tap - kh * 3;
-              const uint64_t bt = bd + (uint64_t)((kh * 10 + kw) * 8);
-#pragma unroll
-              for (int k = 0; k < 8; ++k)
-                umma_f16(d_tmem, ad + (uint64_t)(k * 128), bt + (uint64_t)(k * 160), idesc, k ? 1u : acc);
-            }
-            umma_commit(&b_empty[b_slot]);
-            umma_commit(&a_empty[a_slot]);
-            if (++b_slot == p.b_slots) { b_slot = 0; b_phase ^= 1; }
-            if (++a_slot == 2) { a_slot = 0; a_phase ^= 1; }
-            acc = 1;
-            continue;
-          }
-          uint32_t d_tmem = tmem_base;
-          for (int tap = tap0; tap < tap1; ++tap, d_tmem += Nn) {
-            mbar_wait(&b_full[b_slot], b_phase);
-            tc_fence_after();
-            const uint64_t bd = bd_tmpl + (uint64_t)(b0 + (uint32_t)b_slot * bslot16);
-#pragma unroll
-            for (int k = 0; k < 8; ++k)
-              umma_f16(d_tmem, ad + (uint64_t)(k * 128), bd + (uint64_t)(k * 128), idesc, k ? 1u : acc);
-            umma_commit(&b_empty[b_slot]);
-            if (++b_slot == p.b_slots) { b_slot = 0; b_phase ^= 1; }
-          }
-          umma_commit(&a_empty[a_slot]);
-          if (++a_slot == 2) { a_slot = 0; a_phase ^= 1; }
-          acc = 1;
-        }
-        umma_commit(acc_full);
-      }
-      pdl_launch_late();
-    }
-    __syncwarp();
-  } else if (warp >= 4) {
-    const uint32_t q = warp - 4;
-    int uit = 0;
-    for (int unit = blockIdx.x; unit < p.total_units; unit += gridDim.x, ++uit) {
+  } else {
+    // ------------------------------------------------------------------ consumers: MMA + epilogue
+    const uint32_t g = warp >> 2;              // warpgroup: output channels 64g .. 64g + 63 of the M tile
+    const bool leader = (threadIdx.x & 127) == 0;
+    // 16 pixels per K step = 2048 B of both operands; 8-pixel groups 1024 B apart; 64-channel atoms kABlock apart
+    const uint64_t tmpl = make_smem_desc(0, kABlock, 1024, 1);
+    const uint32_t a0 = smem_u32(a_base) + g * kABlock, b0 = smem_u32(b_base);
+    float acc[NB * 8];
+    int a_slot = 0, b_slot = 0;
+    uint32_t a_phase = 0, b_phase = 0;
+    for (int unit = blockIdx.x; unit < p.total_units; unit += gridDim.x) {
       int m_tile, n_tile, tg, split;
       decode(unit, m_tile, n_tile, tg, split);
       const int n0 = n_tile * p.ntile_w;
-      const int Nn = min(p.ntile_w, p.Cin - n0);
+      const int Nn = min(p.ntile_w, p.Cin - n0);         // multiple of 16
+      const int nb16 = Nn >> 4;
       const int tap0 = tg * p.taps_per_group, tap1 = min(p.taps, tap0 + p.taps_per_group);
-      const bool has_tiles = split < p.pix_tiles;
-      mbar_wait(acc_full, uit & 1);
-      tc_fence_after();
-      const int co = m_tile * 128 + q * 32 + lane;
-      if (has_tiles) {
+      const bool active = g == 0 || (p.Cout - m_tile * 128) > 64;   // this warpgroup's dy block holds real channels
+      PendingRelease pend;
+      uint32_t started = 0;
+      for (int t = split; t < p.pix_tiles; t += p.splits) {
+        mbar_wait(&a_full[a_slot], a_phase);
+        const uint64_t ad = tmpl + (uint64_t)((a0 + (uint32_t)a_slot * (uint32_t)p.a_slot_bytes) >> 4);
         for (int tap = tap0; tap < tap1; ++tap) {
-          for (int ch = 0; ch < Nn / 16; ++ch) {
-            uint32_t r[16];
-            tmem_ld16(tmem_base + ((q * 32u) << 16) + (tap - tap0) * Nn + ch * 16, r);
-            tmem_ld_wait();
-            if (co < p.Cout) {
-              if (p.direct) {
-                // the only unit that touches dw[co][tap][n0 + 16 ch ..]: four 16-byte fire-and-forget reductions
-                float* dst = dw + ((size_t)co * p.taps + tap) * p.Cin + n0 + ch * 16;
+          const int tl = tap - tap0;
+          mbar_wait(&b_full[b_slot], b_phase);
+          const uint64_t bd = tmpl + (uint64_t)((b0 + (uint32_t)b_slot * (uint32_t)p.b_slot_bytes) >> 4);
+          if (active) {
+            wgmma_fence();
+            for (int k = 0; k < 8; ++k) {
 #pragma unroll
-                for (int j = 0; j < 4; ++j)
-                  red_add_v4(dst + 4 * j, __uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]),
-                             __uint_as_float(r[4 * j + 2]), __uint_as_float(r[4 * j + 3]));
-              } else {
-                // per-unit slab [tap_local][128 rows][unit_n] fp32: plain 16-byte stores, summed by wgrad_reduce_kernel
-                float4* dst = reinterpret_cast<float4*>(ws + (size_t)unit * p.unit_stride +
-                                                        ((size_t)(tap - tap0) * 128 + q * 32 + lane) * p.unit_n + ch * 16);
-                dst[0] = make_float4(__uint_as_float(r[0]), __uint_as_float(r[1]), __uint_as_float(r[2]), __uint_as_float(r[3]));
-                dst[1] = make_float4(__uint_as_float(r[4]), __uint_as_float(r[5]), __uint_as_float(r[6]), __uint_as_float(r[7]));
-                dst[2] = make_float4(__uint_as_float(r[8]), __uint_as_float(r[9]), __uint_as_float(r[10]), __uint_as_float(r[11]));
-                dst[3] = make_float4(__uint_as_float(r[12]), __uint_as_float(r[13]), __uint_as_float(r[14]), __uint_as_float(r[15]));
+              for (int j = 0; j < NB; ++j) {
+                const int c = j - tl * nb16;
+                if (c >= 0 && c < nb16 && (c & 3) == 0)
+                  wgmma_mn(&acc[8 * j], nb16 - c, ad + (uint64_t)(k * 128),
+                           bd + (uint64_t)(k * 128 + (c >> 2) * (kABlock >> 4)), started | (uint32_t)k);
               }
+            }
+            wgmma_commit();
+            wgmma_wait<1>();
+          }
+          pend.release(leader);
+          pend.bar0 = &b_empty[b_slot];
+          if (tap == tap1 - 1) pend.bar1 = &a_empty[a_slot];
+          if (++b_slot == p.b_slots) { b_slot = 0; b_phase ^= 1; }
+        }
+        if (++a_slot == 2) { a_slot = 0; a_phase ^= 1; }
+        started = 1;
+      }
+      wgmma_wait<0>();
+      pend.release(leader);
+      if (!started || !active) continue;
+      // thread rows: output channels co0 (+8); block j = (tap tl, 16 columns c): columns 16c + 8h + 2(lane % 4) + {0, 1}
+      const int row0 = (int)(g * 64 + (warp & 3) * 16 + (lane >> 2));
+#pragma unroll
+      for (int j = 0; j < NB; ++j) {
+        if (j >= (tap1 - tap0) * nb16) break;
+        const int tl = j / nb16, c = j - tl * nb16;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int col = c * 16 + 8 * h + 2 * (int)(lane & 3);
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            const int row = row0 + 8 * r, co = m_tile * 128 + row;
+            if (co >= p.Cout) continue;
+            const float v0 = acc[8 * j + 4 * h + 2 * r], v1 = acc[8 * j + 4 * h + 2 * r + 1];
+            if (p.direct) {
+              // the only unit that touches these gradient elements: fire-and-forget reductions
+              float* dst = dw + ((size_t)co * p.taps + tap0 + tl) * p.Cin + n0 + col;
+              atomicAdd(dst, v0);
+              atomicAdd(dst + 1, v1);
+            } else {
+              // per-unit slab [tap_local][128 rows][unit_n] fp32, summed by wgrad_reduce_kernel
+              float2* dst = reinterpret_cast<float2*>(ws + (size_t)unit * p.unit_stride +
+                                                      ((size_t)tl * 128 + row) * p.unit_n + col);
+              *dst = make_float2(v0, v1);
             }
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(acc_empty);
     }
+    if (g == 0 && leader) pdl_launch_late();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) { tc_fence_after(); tmem_dealloc(tmem_base, p.tmem_cols); }
 }
 
 
@@ -381,18 +343,6 @@ publish_grads_kernel(float* __restrict__ dst, const float* __restrict__ src, lon
 
 using namespace b200seg;
 
-// Narrow layers (Cout <= 64, one 64-channel block of x per N tile: the 48 / 64-channel high-resolution branch and the
-// stem) run in a configuration that can share an SM with a co-resident convolution CTA or another weight-gradient CTA:
-// at most 256 TMEM columns (more, smaller tap groups), one 16 KB dy block per stage and a shared-memory footprint below
-// half an SM. A full-SM weight-gradient CTA (512 columns, > 200 KB) excludes every other tensor-core CTA from its SM
-// and vice versa; measured on the two-scale step: 38.37 vs 38.93 ms (profiles/r2_ab_switches.txt).
-// B200SEG_WGRAD_CORES=0 restores the full-SM configuration everywhere.
-static bool wgrad_coresident_enabled() {
-  static const bool on = []() { const char* e = getenv("B200SEG_WGRAD_CORES"); return !(e && e[0] == '0'); }();
-  return on;
-}
-constexpr size_t kWgradHalfSm = 115712;   // (228 KB - 2 x 1 KB reserved) / 2
-
 static int wgrad_plan(const b200seg_conv_desc* d, WgradParams& p) {
   if (!d) return B200SEG_E_BADARG;
   const int dil = d->dilation > 1 ? d->dilation : 1;
@@ -404,10 +354,8 @@ static int wgrad_plan(const b200seg_conv_desc* d, WgradParams& p) {
   p.ksize = d->ksize; p.stride = d->stride; p.pad = d->pad; p.taps = d->ksize * d->ksize; p.dil = dil;
   p.Ho = (d->h + 2 * d->pad - dil * (d->ksize - 1) - 1) / d->stride + 1;
   p.Wo = (d->w + 2 * d->pad - dil * (d->ksize - 1) - 1) / d->stride + 1;
-  p.halo = (d->ksize == 3 && d->stride == 1 && d->reserved == 0 && dil == 1) ? 1 : 0;
-  p.b_block_bytes = p.halo ? 24576 : kABlock;
   p.TW = 16; p.TH = 8;
-  if (p.Wo <= 8 || p.halo) { p.TW = 8; p.TH = 16; }
+  if (p.Wo <= 8) { p.TW = 8; p.TH = 16; }
   p.tiles_w = (p.Wo + p.TW - 1) / p.TW;
   p.tiles_h = (p.Ho + p.TH - 1) / p.TH;
   p.pix_tiles = d->n * p.tiles_h * p.tiles_w;
@@ -422,13 +370,11 @@ static int wgrad_plan(const b200seg_conv_desc* d, WgradParams& p) {
   const int widths[3] = {64, 128, 256};
   for (int wi = 0; wi < 3; ++wi) {
     const int ntw = widths[wi];
-    if (p.halo && ntw > 128) continue;                       // halo B slot: <= 2 blocks of 24 KB
     if (wi > 0 && d->cin <= widths[wi - 1]) continue;        // same tiling as the narrower candidate
     const int n_tiles = (d->cin + ntw - 1) / ntw;
     const int Nmax = d->cin < ntw ? d->cin : ntw;
     const int nblk = (Nmax + 63) / 64;
-    const bool cores = wgrad_coresident_enabled() && d->cout <= 64 && ntw == 64;
-    int tpg_max = (cores ? 256 : 512) / Nmax;
+    int tpg_max = kWAccCols / Nmax;
     if (tpg_max > p.taps) tpg_max = p.taps;
     for (int tg = (p.taps + tpg_max - 1) / tpg_max; tg <= p.taps; ++tg) {
       const int tpg = (p.taps + tg - 1) / tg;
@@ -438,7 +384,7 @@ static int wgrad_plan(const b200seg_conv_desc* d, WgradParams& p) {
       if (sp_max > p.pix_tiles) sp_max = p.pix_tiles;
       if (sp_max < 1) sp_max = 1;
       const double mma = (double)tpg * 8.0 * (Nmax / 2 > 32 ? Nmax / 2 : 32);
-      const double bytes = (a_two ? 32768.0 : 16384.0) + (p.halo ? nblk * 23040.0 : (double)tpg * nblk * 16384.0);
+      const double bytes = (a_two ? 32768.0 : 16384.0) + (double)tpg * nblk * 16384.0;
       const double per_tile = mma > bytes / 64.0 ? mma : bytes / 64.0;
       if (tune().wgrad_min_clk > 0) {     // every unit reduces at least wgrad_min_clk modelled clocks of pixel tiles
         int sp_w = (int)((double)p.pix_tiles * per_tile / (double)tune().wgrad_min_clk);
@@ -474,14 +420,7 @@ static int wgrad_plan(const b200seg_conv_desc* d, WgradParams& p) {
   p.unit_n = Nmax;
   p.unit_stride = (long long)p.taps_per_group * 128 * Nmax;
   p.a_slot_bytes = 2 * kABlock;
-  p.b_slot_bytes = p.nblocksB_max * p.b_block_bytes;
-  p.tmem_cols = 512;
-  if (wgrad_coresident_enabled() && d->cout <= 64 && p.ntile_w == 64 && p.taps_per_group * Nmax <= 256) {
-    p.a_slot_bytes = kABlock;                    // Cout <= 64: the second dy block is never loaded
-    int cols = 32;
-    while (cols < p.taps_per_group * Nmax) cols *= 2;
-    p.tmem_cols = cols;
-  }
+  p.b_slot_bytes = p.nblocksB_max * kABlock;
   return 0;
 }
 
@@ -504,15 +443,14 @@ extern "C" int b200seg_conv2d_wgrad(const b200seg_conv_desc* d, const void* x, c
     if (!workspace || ws_bytes < (size_t)p.total_units * p.unit_stride * sizeof(float)) return B200SEG_E_BADARG;
     if (reinterpret_cast<uintptr_t>(workspace) & 15) return B200SEG_E_BADARG;
   }
-  const size_t fixed = 1024 + 2 * (size_t)p.a_slot_bytes + (4 + 2 * kMaxBSlots + 2) * 8 + 16;
-  const bool cores = p.tmem_cols <= 256;
-  const size_t budget = cores ? kWgradHalfSm - (size_t)smem_reserve() / 2 : (size_t)227 * 1024 - smem_reserve();
+  const size_t fixed = 1024 + 2 * (size_t)p.a_slot_bytes + (4 + 2 * kMaxBSlots) * 8 + 16;
+  const size_t budget = (size_t)227 * 1024 - smem_reserve();
   int bs = (int)((budget - fixed) / p.b_slot_bytes);
   if (bs > kMaxBSlots) bs = kMaxBSlots;
   if (bs < 2) return B200SEG_E_BADARG;
   p.b_slots = bs;
   size_t smem_bytes = fixed + (size_t)bs * p.b_slot_bytes;
-  if (!cores && smem_bytes < 120 * 1024) smem_bytes = 120 * 1024;      // one CTA per SM
+  if (smem_bytes < 120 * 1024) smem_bytes = 120 * 1024;      // one CTA per SM
 
   CUtensorMap tmDy, tmX;
   {
@@ -526,7 +464,6 @@ extern "C" int b200seg_conv2d_wgrad(const b200seg_conv_desc* d, const void* x, c
     uint64_t dims[4] = {(uint64_t)d->cin, (uint64_t)d->w, (uint64_t)d->h, (uint64_t)d->n};
     uint64_t strides[3] = {(uint64_t)d->x_ld * 2, (uint64_t)d->w * d->x_ld * 2, (uint64_t)d->h * d->w * d->x_ld * 2};
     uint32_t box[4] = {64, (uint32_t)(p.TW * d->stride), (uint32_t)(p.TH * d->stride), 1};
-    if (p.halo) { box[1] = 10; box[2] = 18; }
     uint32_t es[4] = {1, (uint32_t)d->stride, (uint32_t)d->stride, 1};
     int rc = encode_bf16(&tmX, x, 4, dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
@@ -576,7 +513,7 @@ extern "C" int b200seg_publish_grads(float* dst, const float* src, int64_t n, co
   if (!dst || !src || n <= 0 || (n & 3) || (reinterpret_cast<uintptr_t>(dst) & 15) ||
       (reinterpret_cast<uintptr_t>(src) & 15))
     return B200SEG_E_BADARG;
-  cudaError_t e = launch_k(publish_grads_kernel, dim3(148 * 8), dim3(256), 0, (cudaStream_t)stream, dst, src,
+  cudaError_t e = launch_k(publish_grads_kernel, dim3(B200SEG_MAX_CTAS * 8), dim3(256), 0, (cudaStream_t)stream, dst, src,
                            (long long)(n / 4), scale_dev, scale_const, (int)accumulate);
   return e == cudaSuccess ? 0 : (int)e;
 }

@@ -1,4 +1,4 @@
-"""network.basic factory (network/basic.py:104) backed by the sm_100a kernels (BASELINE config 1 plumbing model)."""
+"""network.basic factory (network/basic.py:104) backed by the sm_90a kernels (BASELINE config 1 plumbing model)."""
 from ._factory import build
 
 

@@ -1,4 +1,4 @@
-"""network.deepv3 factory (network/deepv3.py:165-170) backed by the sm_100a kernels (SURVEY.md §8 row f2)."""
+"""network.deepv3 factory (network/deepv3.py:165-170) backed by the sm_90a kernels (SURVEY.md §8 row f2)."""
 from ._factory import build
 
 

@@ -1,4 +1,4 @@
-"""network.ocrnet factories (network/ocrnet.py:337-342) backed by the sm_100a kernels."""
+"""network.ocrnet factories (network/ocrnet.py:337-342) backed by the sm_90a kernels."""
 from ._factory import build
 
 

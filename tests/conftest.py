@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "semantic-segmentation_b200")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run with -m gpu on a B200)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run with -m gpu on an H100)")
 
 
 @pytest.fixture(scope="session")

@@ -1,6 +1,6 @@
 """Host-only sweep of the convolution launch planner (b200seg_conv2d_plan_info) over every convolution shape of the
 W48 two-scale step (both passes) and of the reduced test networks: shared memory within the per-SM limits for the chosen
-occupancy, TMEM columns a power of two that fits the SM, rings deep enough to pipeline, grids within the slot count."""
+occupancy, accumulators that fit the register budget of that occupancy, rings deep enough to pipeline, grids within the slot count."""
 import ctypes
 
 import pytest
@@ -62,14 +62,15 @@ def test_every_model_convolution_has_a_valid_plan(which):
         d = _desc(n, h, w, cin, cout, k, stride, emit_stats=1 if which == 0 else 0)
         rc = L.b200seg_conv2d_plan_info(ctypes.byref(d), which, out)
         assert rc == 0, (n, h, w, cin, cout, k, stride, rc)
-        kern, bn, nt, grid, smem, depth, occ, tmem, resident, bslots = list(out)
+        kern, bn, nt, grid, smem, depth, occ, acc_regs, resident, bslots = list(out)
         key = (n, h, w, cin, cout, k, stride)
         seen.add((kern, occ))
-        assert occ in (1, 2) and 1 <= grid <= 148 * occ, key
-        assert tmem in (64, 128, 256, 512) and tmem >= 2 * bn and occ * tmem <= 512, (key, tmem, bn)
+        assert occ in (1, 2) and 1 <= grid <= 132 * occ, key
+        # fp32 accumulators per consumer thread: 64 rows x BN columns over 128 threads; two CTAs per SM hold <= 64 each
+        assert acc_regs == bn // 2 and occ * acc_regs <= 128, (key, acc_regs, bn)
         assert smem <= CTA_SMEM and occ * (smem + 1024) <= SM_SMEM, (key, smem, occ)
         if occ == 1:
-            assert 2 * (smem + 1024) > SM_SMEM, (key, smem)      # a second CTA can never slip in next to a 512-column one
+            assert 2 * (smem + 1024) > SM_SMEM, (key, smem)      # a second CTA can never slip in next to a full-SM one
         assert bn % 16 == 0 and bn <= 256 and nt * bn >= (cout if which == 0 else cin), key
         if kern == 1:
             assert depth >= 2 and (resident == 1 or bslots >= 2), key

@@ -1,4 +1,4 @@
-"""SURVEY §8(f) row f2: deepv3.DeepV3PlusW38 (WideResNet-38 trunk, ASPP, decoder) on the sm_100a kernels against the
+"""SURVEY §8(f) row f2: deepv3.DeepV3PlusW38 (WideResNet-38 trunk, ASPP, decoder) on the sm_90a kernels against the
 oracle restatement (oracle/seg_oracle.py deepv3_forward, pinned to the reference by tests/test_oracle_golden.py).
 A reduced-width WRN keeps the oracle at seconds; the structure (pools, stride, dilations 2/4, bottleneck blocks,
 dilated ASPP 12/24/36, image pooling, 304-channel decoder concat) is the full one."""

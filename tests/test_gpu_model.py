@@ -219,6 +219,29 @@ def test_cuda_graph_replay_equals_eager():
         assert abs(losses[0] - losses[1]) <= 2e-3 * abs(losses[0]), (step, losses)
 
 
+def test_train_step_is_bitwise_reproducible():
+    """Two runs of one step on the same weights and batch: identical loss and gradients (fixed summation orders)."""
+    O, B200SegModule = _mods()
+    hcfg = O.HRNET_W16_TEST
+    arch = "ocrnet.HRNet_Mscale"
+    sd0 = O.synth_state_dict(arch, hcfg, seed=3)
+    ocfg = dict(O.OCR_CFG)
+    ocfg["dropout"] = 0.0
+    images, gts = O.synth_batch(2, 64, 128, seed=7)
+    runs = []
+    for _ in range(2):
+        net = B200SegModule(arch, 19, hcfg=hcfg, ocfg=ocfg, use_cuda_graph=False)
+        net.load_state_dict(sd0)
+        net = net.cuda().train()
+        loss = net({"images": images.cuda(), "gts": gts.cuda()})
+        loss.backward()
+        runs.append((float(loss), {n: p.grad.detach().clone() for n, p in net.named_parameters() if p.grad is not None}))
+    assert runs[0][0] == runs[1][0], (runs[0][0], runs[1][0])
+    assert runs[0][1].keys() == runs[1][1].keys()
+    differ = [n for n in runs[0][1] if not torch.equal(runs[0][1][n], runs[1][1][n])]
+    assert not differ, differ[:8]
+
+
 def _condition_eval_weights(sd0):
     """Randomly initialised heads produce soft-region logits of magnitude ~150 and attention logits of ~1e3: both feed a
     softmax, so a 1 % bf16 difference in a logit changes a probability by e^1.5 and an eval comparison against ANY

@@ -310,7 +310,11 @@ def test_batchnorm_train_fwd_bwd(c, res, relu, size):
     if res:
         o = o + rr
     if relu:
-        o = F.relu(o)
+        # a pre-activation that is zero up to fp32 summation order lies on either side of the ReLU: there the mask is the
+        # side the kernel's forward took (its output z is checked against this reference just below)
+        pre = o.detach()
+        tie = pre.abs() <= 1e-6 * pre.abs().max()
+        o = o * torch.where(tie, z.float().permute(0, 3, 1, 2) > 0, pre > 0)
     o = o * ps[:, :, None, None]
     close(z, o.permute(0, 2, 3, 1), BF16_TOL, "bn fwd")
     close(rm, rm2, 1e-4, "running mean")

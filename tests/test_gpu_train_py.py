@@ -1,5 +1,6 @@
-"""Boundary proof (SURVEY.md §8b): the UNMODIFIED reference train.py (baseline/_ref/semantic-segmentation/train.py, a
-verbatim copy of the reference checkout made by __graft_entry__.build()) runs on the overlay: `import network` resolves to
+"""Boundary proof (SURVEY.md §8b): the UNMODIFIED reference train.py (oracle/_ref/semantic-segmentation/train.py, a
+verbatim copy of the reference checkout made by oracle/reference_build.py in __graft_entry__.build()) runs on the
+overlay: `import network` resolves to
 semantic-segmentation_b200/network, network.get_net / wrap_network_in_dataparallel / optimizer / validate / checkpoint
 code of the reference run unchanged (train.py:377-383, 488-509, utils/trnval_utils.py), the loss is finite and does not
 increase on the (constant) nullloader batch, and the checkpoint logx.save_model wrote is restored by --snapshot."""
@@ -14,7 +15,7 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref", "semantic-segmentation")
+REF = os.path.join(ROOT, "oracle", "_ref", "semantic-segmentation")
 PKG = os.path.join(ROOT, "semantic-segmentation_b200")
 
 
@@ -33,7 +34,7 @@ def _run(args, cwd):
                                        ("mscale.HRNet", "128,256")])
 def test_reference_train_py_runs_unchanged_on_the_overlay(tmp_path, arch, crop):
     if not os.path.isfile(os.path.join(REF, "train.py")):
-        pytest.skip("baseline/_ref/semantic-segmentation is absent (run __graft_entry__.build() where /root/reference exists)")
+        pytest.skip("oracle/_ref/semantic-segmentation is absent (__graft_entry__.build() with a reference checkout)")
     logs = str(tmp_path / "logs")
     common = ["--dataset", "nullloader", "--arch", arch, "--crop_size", crop, "--bs_trn", "1", "--bs_val", "1",
               "--class_uniform_pct", "0", "--num_workers", "0", "--test_mode", "--result_dir", logs]

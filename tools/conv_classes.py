@@ -1,9 +1,9 @@
 """Joins the static step trace (tools/trace_step.py: shapes, FLOPs, bytes of every convolution launch, program order) with
-an ncu launch list of the same step (profiles/*.csv.gz: measured duration of every kernel, launch order) and prints, per
+an ncu launch list of the same step (a .csv.gz: measured duration of every kernel, launch order) and prints, per
 convolution class (kind, shape), launches, measured time, roofline time and their ratio. The launch list starts somewhere
 inside a step, so the expected kernel-name sequence is rotated onto the observed one first.
 
-    python -O tools/conv_classes.py profiles/r1_launches_v2.csv.gz
+    python -O tools/conv_classes.py launches.csv.gz
     python -O tools/conv_classes.py gpurun_out/abi_launches.csv --abi gpurun_out/abi_calls.json
 
 With --abi (the log tools/gpu_abi_log.py wrote in the SAME run as the launch list) nothing is guessed: the k-th b200seg

@@ -30,7 +30,7 @@ for (h, w, c) in shapes:
     w1f, _ = raw.pack_weight(w1)
     dw = torch.zeros_like(wt)
     y = torch.empty_like(x)
-    stats = torch.empty(148 * 2 * 1024, device="cuda")
+    stats = torch.empty(264 * 2 * 1024, device="cuda")
     scale = torch.ones(c, device="cuda"); shift = torch.zeros(c, device="cuda")
     import ctypes
     from b200seg._lib import lib, ptr, stream_ptr

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """SM-time view of ONE training step from an `ncu --metrics gpu__time_duration.sum` launch list (csv or csv.gz):
 per kernel family the summed durations and the same weighted by the share of the GPU the launch can hold
-(grid / (148 x CTAs per SM of that kernel)). If the weighted sum is close to the measured step time the step is bound by
+(grid / (132 x CTAs per SM of that kernel)). If the weighted sum is close to the measured step time the step is bound by
 SM occupancy (every launch that takes the whole GPU excludes the other streams), not by launch rate or by any single
-chain's latency. usage: python tools/sm_time.py profiles/r2_launches_step.csv.gz"""
+chain's latency. usage: python tools/sm_time.py launches.csv.gz"""
 import collections
 import csv
 import gzip
@@ -32,10 +32,10 @@ def prod(field, d):
 
 def share(nm, grid, block):
     if "halo_kernel<2" in nm or "igemm_kernel<2" in nm:      # two co-resident CTAs fill an SM (registers, shared memory)
-        return min(1.0, grid / 296.0)
+        return min(1.0, grid / 264.0)
     if "halo_kernel<1" in nm or "conv_igemm_kernel<1" in nm or "wgrad_igemm" in nm:   # one CTA owns its SM
-        return min(1.0, grid / 148.0)
-    return min(1.0, grid / (148.0 * max(1, 2048 // block)))  # thread-slot share of the CUDA-core kernels
+        return min(1.0, grid / 132.0)
+    return min(1.0, grid / (132.0 * max(1, 2048 // block)))  # thread-slot share of the CUDA-core kernels
 
 
 agg = collections.defaultdict(lambda: [0, 0.0, 0.0])
