@@ -55,9 +55,16 @@ typedef struct b200seg_conv_desc {
 } b200seg_conv_desc;
 
 /* Host-only introspection of the launch plan (tests, tuning): which = 0 forward, 1 stride-1 data gradient.
- * out[10] = {kernel (1 = halo-tile 3x3, 0 = per-tap implicit GEMM), Cout tile, Cout tiles, grid, dynamic shared memory
- * bytes, ring depth, CTAs per SM, accumulator registers per thread, resident weights, weight slots}. Returns 0 or a negative error. */
+ * out[12] = {kernel (1 = halo-tile 3x3, 0 = per-tap implicit GEMM), Cout tile, Cout tiles, grid, dynamic shared memory
+ * bytes, ring depth, CTAs per SM, accumulator registers per thread, resident weights, weight slots, channel chunk per
+ * pipeline stage (16/32/64), tiles (pixel tiles x Cout tiles)}. Returns 0 or a negative error. */
 int b200seg_conv2d_plan_info(const b200seg_conv_desc* d, int32_t which, int32_t* out);
+
+/* Host-only introspection of the weight-gradient plan (b200seg_conv2d_wgrad): out[10] = {N tile width in input channels
+ * (64/128/256), N tiles, taps per group, tap groups, pixel splits (1 = direct: every gradient element owned by one work
+ * unit, no workspace), M tiles (128 output channels), work units, grid, B-ring slots, dynamic shared memory bytes}.
+ * Returns 0 or a negative error. */
+int b200seg_conv2d_wgrad_plan_info(const b200seg_conv_desc* d, int32_t* out);
 
 /* Diagnostics (needs a GPU): CTAs per SM the runtime grants kernel (1 = halo-tile 3x3, 0 = per-tap) in its
  * co-resident (occ_variant 2) or full-SM (1) build with smem_bytes of dynamic shared memory; negative = error. */

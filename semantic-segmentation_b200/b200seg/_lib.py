@@ -73,6 +73,7 @@ SIGNATURES = {
     "b200seg_build_info": (ctypes.c_char_p, []),
     "b200seg_conv2d_stats_elems": (c_size_t, [ctypes.POINTER(ConvDesc)]),
     "b200seg_conv2d_plan_info": (c_int32, [ctypes.POINTER(ConvDesc), c_int32, P32]),
+    "b200seg_conv2d_wgrad_plan_info": (c_int32, [ctypes.POINTER(ConvDesc), P32]),
     "b200seg_debug_occupancy": (c_int32, [c_int32, c_int32, c_int32]),
     "b200seg_debug_occupancy_report": (None, []),
     "b200seg_conv2d_fwd": (ctypes.c_int, [ctypes.POINTER(ConvDesc), V, V, V, V, V, P32, V]),

@@ -307,14 +307,14 @@ static int halo_plan(int n, int h, int w, int cin, int cout, HaloParams& p, size
 }
 
 // {kernel 1 = halo, BN, n_tiles, grid, smem bytes, ring depth (A slots), CTAs per SM, accumulator registers per consumer
-// thread, resident weights, B slots}
+// thread, resident weights, B slots, channel chunk (64), total tiles}
 int conv3x3_halo_plan_info(int n, int h, int w, int cin, int cout, int32_t* out) {
   HaloParams p;
   size_t smem_bytes;
   int grid, occ;
   if (int rc = halo_plan(n, h, w, cin, cout, p, smem_bytes, grid, occ)) return rc;
   out[0] = 1; out[1] = p.BN; out[2] = p.n_tiles; out[3] = grid; out[4] = (int32_t)smem_bytes; out[5] = p.a_slots;
-  out[6] = occ; out[7] = p.BN / 2; out[8] = p.resident; out[9] = p.b_slots;
+  out[6] = occ; out[7] = p.BN / 2; out[8] = p.resident; out[9] = p.b_slots; out[10] = 64; out[11] = p.total_tiles;
   return 0;
 }
 

@@ -454,8 +454,8 @@ extern "C" size_t b200seg_conv2d_stats_elems(const b200seg_conv_desc* d) {
 }
 
 // Host-only: the launch plan of a forward (which = 0) or stride-1 data-gradient (which = 1) convolution, for tests and
-// tuning scripts. out[10] = {kernel (1 halo / 0 per-tap), BN, n_tiles, grid, dynamic smem bytes, ring depth, CTAs per SM,
-// accumulator registers per consumer thread, resident weights (halo), weight slots (halo)}.
+// tuning scripts. out[12] = {kernel (1 halo / 0 per-tap), BN, n_tiles, grid, dynamic smem bytes, ring depth, CTAs per SM,
+// accumulator registers per consumer thread, resident weights (halo), weight slots (halo), channel chunk, total tiles}.
 extern "C" int b200seg_conv2d_plan_info(const b200seg_conv_desc* d, int32_t which, int32_t* out) {
   if (!desc_ok(d) || !out || which < 0 || which > 1) return B200SEG_E_BADARG;
   if (which == 1 && d->stride != 1) return B200SEG_E_BADARG;
@@ -471,7 +471,7 @@ extern "C" int b200seg_conv2d_plan_info(const b200seg_conv_desc* d, int32_t whic
   ConvPlan pl;
   if (int rc = plan_geom(g, &pl)) return rc;
   out[0] = 0; out[1] = pl.BN; out[2] = pl.n_tiles; out[3] = pl.grid; out[4] = (int32_t)pl.smem_bytes; out[5] = pl.nstages;
-  out[6] = pl.occ; out[7] = pl.acc_regs; out[8] = 0; out[9] = 0;
+  out[6] = pl.occ; out[7] = pl.acc_regs; out[8] = 0; out[9] = 0; out[10] = pl.KC; out[11] = pl.total_tiles;
   return 0;
 }
 

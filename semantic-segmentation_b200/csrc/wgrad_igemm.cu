@@ -343,7 +343,11 @@ publish_grads_kernel(float* __restrict__ dst, const float* __restrict__ src, lon
 
 using namespace b200seg;
 
-static int wgrad_plan(const b200seg_conv_desc* d, WgradParams& p) {
+static int wgrad_grid(const WgradParams& p) { return p.total_units < B200SEG_MAX_CTAS ? p.total_units : B200SEG_MAX_CTAS; }
+
+// Decomposition, B-ring depth and dynamic shared memory of one launch (host only; also reported by
+// b200seg_conv2d_wgrad_plan_info, so the query and the launch cannot disagree).
+static int wgrad_plan(const b200seg_conv_desc* d, WgradParams& p, size_t& smem_bytes) {
   if (!d) return B200SEG_E_BADARG;
   const int dil = d->dilation > 1 ? d->dilation : 1;
   if (!((d->ksize == 1 && d->pad == 0 && dil == 1) || (d->ksize == 3 && d->pad == dil))) return B200SEG_E_BADARG;
@@ -421,12 +425,32 @@ static int wgrad_plan(const b200seg_conv_desc* d, WgradParams& p) {
   p.unit_stride = (long long)p.taps_per_group * 128 * Nmax;
   p.a_slot_bytes = 2 * kABlock;
   p.b_slot_bytes = p.nblocksB_max * kABlock;
+  const size_t fixed = 1024 + 2 * (size_t)p.a_slot_bytes + (4 + 2 * kMaxBSlots) * 8 + 16;
+  const size_t budget = (size_t)227 * 1024 - smem_reserve();
+  int bs = (int)((budget - fixed) / p.b_slot_bytes);
+  if (bs > kMaxBSlots) bs = kMaxBSlots;
+  if (bs < 2) return B200SEG_E_BADARG;
+  p.b_slots = bs;
+  smem_bytes = fixed + (size_t)bs * p.b_slot_bytes;
+  if (smem_bytes < 120 * 1024) smem_bytes = 120 * 1024;      // one CTA per SM
+  return 0;
+}
+
+extern "C" int b200seg_conv2d_wgrad_plan_info(const b200seg_conv_desc* d, int32_t* out) {
+  WgradParams p;
+  size_t smem_bytes;
+  if (!out) return B200SEG_E_BADARG;
+  if (int rc = wgrad_plan(d, p, smem_bytes)) return rc;
+  out[0] = p.ntile_w; out[1] = p.n_tiles; out[2] = p.taps_per_group; out[3] = p.tap_groups; out[4] = p.splits;
+  out[5] = p.m_tiles; out[6] = p.total_units; out[7] = wgrad_grid(p);
+  out[8] = p.b_slots; out[9] = (int32_t)smem_bytes;
   return 0;
 }
 
 extern "C" size_t b200seg_conv2d_wgrad_ws_bytes(const b200seg_conv_desc* d) {
   WgradParams p;
-  if (wgrad_plan(d, p) != 0) return 0;
+  size_t smem_bytes;
+  if (wgrad_plan(d, p, smem_bytes) != 0) return 0;
   if (p.direct) return 16;   // no slabs: the workspace is not touched (a non-zero size keeps callers' allocation uniform)
   return (size_t)p.total_units * p.unit_stride * sizeof(float);
 }
@@ -436,21 +460,14 @@ extern "C" int b200seg_conv2d_wgrad(const b200seg_conv_desc* d, const void* x, c
   if (!d || !x || !dy || !dw_ohwi) return B200SEG_E_BADARG;
   if (dy_ld % 8 || dy_ld < 8) return B200SEG_E_BADARG;
   WgradParams p;
-  int rc0 = wgrad_plan(d, p);
+  size_t smem_bytes;
+  int rc0 = wgrad_plan(d, p, smem_bytes);
   if (rc0) return rc0;
   if (reinterpret_cast<uintptr_t>(dw_ohwi) & 15) return B200SEG_E_BADARG;
   if (!p.direct) {
     if (!workspace || ws_bytes < (size_t)p.total_units * p.unit_stride * sizeof(float)) return B200SEG_E_BADARG;
     if (reinterpret_cast<uintptr_t>(workspace) & 15) return B200SEG_E_BADARG;
   }
-  const size_t fixed = 1024 + 2 * (size_t)p.a_slot_bytes + (4 + 2 * kMaxBSlots) * 8 + 16;
-  const size_t budget = (size_t)227 * 1024 - smem_reserve();
-  int bs = (int)((budget - fixed) / p.b_slot_bytes);
-  if (bs > kMaxBSlots) bs = kMaxBSlots;
-  if (bs < 2) return B200SEG_E_BADARG;
-  p.b_slots = bs;
-  size_t smem_bytes = fixed + (size_t)bs * p.b_slot_bytes;
-  if (smem_bytes < 120 * 1024) smem_bytes = 120 * 1024;      // one CTA per SM
 
   CUtensorMap tmDy, tmX;
   {
@@ -476,8 +493,7 @@ extern "C" int b200seg_conv2d_wgrad(const b200seg_conv_desc* d, const void* x, c
     if (e != cudaSuccess) return (int)e;
     attr_set = true;
   }
-  const int grid = p.total_units < B200SEG_MAX_CTAS ? p.total_units : B200SEG_MAX_CTAS;
-  cudaError_t e = launch_k(wgrad_igemm_kernel, dim3(grid), dim3(kWThreads), smem_bytes, (cudaStream_t)stream, tmDy,
+  cudaError_t e = launch_k(wgrad_igemm_kernel, dim3(wgrad_grid(p)), dim3(kWThreads), smem_bytes, (cudaStream_t)stream, tmDy,
                            tmX, p, (float*)workspace, dw_ohwi);
   if (e != cudaSuccess) return (int)e;
   if (p.direct) return 0;
@@ -493,7 +509,8 @@ extern "C" int b200seg_conv2d_wgrad(const b200seg_conv_desc* d, const void* x, c
 /* number of kernels b200seg_conv2d_wgrad launches for this shape (1: direct, 2: split + reduce) */
 extern "C" int32_t b200seg_conv2d_wgrad_launches(const b200seg_conv_desc* d) {
   WgradParams p;
-  if (wgrad_plan(d, p) != 0) return 0;
+  size_t smem_bytes;
+  if (wgrad_plan(d, p, smem_bytes) != 0) return 0;
   return p.direct ? 1 : 2;
 }
 

@@ -1,11 +1,21 @@
-"""Host-only sweep of the convolution launch planner (b200seg_conv2d_plan_info) over every convolution shape of the
-W48 two-scale step (both passes) and of the reduced test networks: shared memory within the per-SM limits for the chosen
-occupancy, accumulators that fit the register budget of that occupancy, rings deep enough to pipeline, grids within the slot count."""
+"""Host-only sweep of the convolution launch planners (b200seg_conv2d_plan_info, b200seg_conv2d_wgrad_plan_info) over
+every convolution shape of the W48 two-scale step (both passes) and of the reduced test networks: shared memory within the
+per-SM limits for the chosen occupancy, accumulators that fit the register budget of that occupancy, rings deep enough to
+pipeline, grids within the slot count. Also checks that the GPU configuration table of tests/test_gpu_conv_classes.py
+still reaches its configurations and covers every configuration the traced step launches."""
 import ctypes
+import json
+import os
+import re
+import subprocess
+import sys
 
 import pytest
 
 from b200seg import _lib
+import test_gpu_conv_classes as classes
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 SM_SMEM = 233472          # 228 KB per SM
 CTA_SMEM = 232448         # 227 KB opt-in maximum per CTA
@@ -54,7 +64,7 @@ CASES = (_hrnet_shapes(1024, 2048) + _hrnet_shapes(512, 1024) + _hrnet_shapes(64
 @pytest.mark.parametrize("which", [0, 1])
 def test_every_model_convolution_has_a_valid_plan(which):
     L = _lib.lib()
-    out = (ctypes.c_int32 * 10)()
+    out = (ctypes.c_int32 * 12)()
     seen = set()
     for (n, h, w, cin, cout, k, stride) in CASES:
         if which == 1 and (stride != 1 or cin == 16):
@@ -62,7 +72,7 @@ def test_every_model_convolution_has_a_valid_plan(which):
         d = _desc(n, h, w, cin, cout, k, stride, emit_stats=1 if which == 0 else 0)
         rc = L.b200seg_conv2d_plan_info(ctypes.byref(d), which, out)
         assert rc == 0, (n, h, w, cin, cout, k, stride, rc)
-        kern, bn, nt, grid, smem, depth, occ, acc_regs, resident, bslots = list(out)
+        kern, bn, nt, grid, smem, depth, occ, acc_regs, resident, bslots, kc, tiles = list(out)
         key = (n, h, w, cin, cout, k, stride)
         seen.add((kern, occ))
         assert occ in (1, 2) and 1 <= grid <= 132 * occ, key
@@ -72,9 +82,80 @@ def test_every_model_convolution_has_a_valid_plan(which):
         if occ == 1:
             assert 2 * (smem + 1024) > SM_SMEM, (key, smem)      # a second CTA can never slip in next to a full-SM one
         assert bn % 16 == 0 and bn <= 256 and nt * bn >= (cout if which == 0 else cin), key
+        assert kc in (16, 32, 64) and tiles % nt == 0 and grid <= tiles, key
         if kern == 1:
             assert depth >= 2 and (resident == 1 or bslots >= 2), key
             assert not (occ == 2 and resident == 0 and bslots < 4), key
         else:
             assert depth >= (3 if occ == 2 else 2), key
     assert (1, 2) in seen and (1, 1) in seen      # both the co-resident and the full-SM configuration are exercised
+
+
+@pytest.mark.parametrize("reserve", [0, classes.SYNCBN_RESERVE])
+def test_every_model_weight_gradient_has_a_valid_plan(reserve):
+    L = _lib.lib()
+    out = (ctypes.c_int32 * 10)()
+    seen = set()
+    with classes.smem_reserve(reserve):
+        for (n, h, w, cin, cout, k, stride) in CASES:
+            key = (n, h, w, cin, cout, k, stride)
+            d = _desc(n, h, w, cin, cout, k, stride)
+            assert L.b200seg_conv2d_wgrad_plan_info(ctypes.byref(d), out) == 0, key
+            ntile, n_tiles, tpg, groups, splits, m_tiles, units, grid, b_slots, smem = list(out)
+            seen.add((ntile, splits == 1))
+            assert ntile in (64, 128, 256) and (n_tiles - 1) * ntile < cin <= n_tiles * ntile, key
+            assert tpg * min(cin, ntile) <= 256 and groups * tpg >= k * k > (groups - 1) * tpg, key
+            assert m_tiles == (cout + 127) // 128 and units == m_tiles * n_tiles * groups * splits, key
+            assert 1 <= grid <= 132 and grid == min(units, 132), key
+            assert 2 <= b_slots <= 6 and smem <= CTA_SMEM - reserve, (key, smem)
+            ws = L.b200seg_conv2d_wgrad_ws_bytes(ctypes.byref(d))
+            assert L.b200seg_conv2d_wgrad_launches(ctypes.byref(d)) == (1 if splits == 1 else 2), key
+            assert (ws == 16) == (splits == 1), key
+    assert {(64, True), (64, False), (128, True), (128, False), (256, False)} <= seen
+
+
+def test_conv_classes_table_plans_to_its_declared_keys():
+    wrong = []
+    for case in classes.CASES:
+        entry, shape, reserve, key = case
+        with classes.smem_reserve(reserve):
+            got = classes.config_key(entry, shape)
+        if got != key:
+            wrong.append("%s declares %s, plans to %s" % (classes._case_id(case), key, got))
+    assert not wrong, "\n".join(wrong)
+
+
+def _step_convolutions():
+    """(entry, (n, h, w, cin, cout, k, stride)) of every tensor-core launch of the traced two-scale W48 step
+    (tools/trace_step.py through tools/conv_classes.py::load_trace, run with -O as the trace requires)."""
+    code = ("import json, sys; sys.path.insert(0, %r); import conv_classes; "
+            "print(json.dumps(sorted(set((kind, detail) for _, kind, detail, _, _ in conv_classes.load_trace()))))"
+            % os.path.join(ROOT, "tools"))
+    res = subprocess.run([sys.executable, "-O", "-c", code], capture_output=True, text=True, timeout=600)
+    assert res.returncode == 0, res.stderr[-2000:]
+    convs = set()
+    for kind, detail in json.loads(res.stdout.strip().splitlines()[-1]):
+        h, w, cin, cout, k, s = map(int, re.match(r"(\d+)x(\d+) c(\d+)->(\d+) k(\d) s(\d)", detail).groups())
+        convs.add((kind, (1, h, w, cin, cout, k, s)))
+    return convs
+
+
+def test_conv_classes_table_covers_every_configuration_of_the_step():
+    convs = _step_convolutions()
+    assert len(convs) > 150 and {kind for kind, _ in convs} == {"fwd", "dgrad", "wgrad"}
+    table = set()
+    for entry, shape, reserve, _key in classes.CASES:
+        with classes.smem_reserve(reserve):
+            table.add((entry, classes.config_key(entry, shape)))
+    missing = []
+    for reserve in (0, classes.SYNCBN_RESERVE):
+        with classes.smem_reserve(reserve):
+            for kind, shape in sorted(convs):
+                if kind == "dgrad" and shape[6] != 1:
+                    continue          # stride-2 data gradients: four sub-lattice launches, listed in EXTRA_CASES
+                key = (kind, classes.config_key(kind, shape))
+                if key not in table:
+                    missing.append("reserve %d: %s %s (step layer %s)" % (reserve, kind, key[1], shape))
+                    table.add(key)
+    assert not missing, "configurations of the step without a case in tests/test_gpu_conv_classes.py:\n" + \
+        "\n".join(missing)

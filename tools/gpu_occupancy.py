@@ -15,7 +15,7 @@ import test_conv_plans as T  # noqa: E402
 
 torch.zeros(1, device="cuda")
 L = _lib.lib()
-out = (ctypes.c_int32 * 10)()
+out = (ctypes.c_int32 * 12)()
 seen = set()
 for case in T._hrnet_shapes(1024, 2048) + T._hrnet_shapes(512, 1024):
     d = T._desc(*case)
