@@ -392,6 +392,28 @@ int b200seg_mscale_loss_fwd(const b200seg_mscale_desc* d, const int64_t* labels,
                             const float* hi_cls, const float* hi_aux, const float* mid, const float* mid_sup, void* g_hi,
                             void* g_lo, void* g_sup, float* partial_ws, float* loss_out, const float* rmi_dpr,
                             const float* rmi_terms, int32_t n_rmi_terms, void* stream);
+/* b200seg_mscale_loss_fwd with two optional extensions (NULL / 0 for either gives b200seg_mscale_loss_fwd's result):
+ * class_coef (loss_kind 0, ImageBasedCrossEntropyLoss2d, loss/utils.py:70-118): fp32 [n][19] per-pixel coefficient of
+ *   the label's class from b200seg_label_class_weights; every head and supervised term is then the sum over images of
+ *   the class-weighted per-image mean, and inv_count must be that call's loss_scale (1, or NaN for an image without a
+ *   valid pixel; the gradient never includes it).
+ * rmi_dpr_aux / rmi_terms_aux (loss_kind 1, nheads 2, cfg.LOSS.OCR_AUX_RMI): the RMI gradient and weighted terms of the
+ *   auxiliary head (b200seg_rmi_pool_aux + b200seg_rmi_solve_grad with scale w_head1 * (1 - lambda) / (n * 9)); its BCE
+ *   weight becomes w_head1 * lambda and loss_out[6] receives the auxiliary RMI term. */
+int b200seg_mscale_loss_fwd_ex(const b200seg_mscale_desc* d, const int64_t* labels, const float* inv_count,
+                               const float* class_coef, const float* hi_cls, const float* hi_aux, const float* mid,
+                               const float* mid_sup, void* g_hi, void* g_lo, void* g_sup, float* partial_ws,
+                               float* loss_out, const float* rmi_dpr, const float* rmi_terms, int32_t n_rmi_terms,
+                               const float* rmi_dpr_aux, const float* rmi_terms_aux, int32_t n_rmi_terms_aux,
+                               void* stream);
+/* ImageBasedCrossEntropyLoss2d.calculate_weights over the whole batch (loss/utils.py:86-99, norm=False): labels int64
+ * [n][per_image]; counts int32 [n][19] exact per-image counts of the labels in [0, 19); weights fp32 [19]
+ * w = (bins != 0) * upper_bound * (1 - bins / sum(bins)) + 1 in fp32 (round_half: rounded through binary16);
+ * coef fp32 [n][19] = w[c] / sum_c w[c] * counts[i][c] (NaN row for an image without a valid pixel);
+ * loss_scale fp32 [1] = 1, or NaN when some image has no valid pixel. Deterministic; two launches and a memset. */
+int b200seg_label_class_weights(const int64_t* labels, int32_t n, int64_t per_image, float upper_bound,
+                                int32_t round_half, int32_t* counts, float* weights, float* coef, float* loss_scale,
+                                void* stream);
 int b200seg_mscale_hi_bwd(const b200seg_mscale_desc* d, const void* g_hi, void* d_cls, void* d_aux, void* stream);
 /* dmid_ws: fp32 [n*hm*wm][40]; d_attn: bf16 [n*hl*wl][8] gradient w.r.t. the PRE-sigmoid attention logit */
 int b200seg_mscale_lo_bwd(const b200seg_mscale_desc* d, const void* g_lo, const void* g_sup, const float* lo_cls,
@@ -406,6 +428,11 @@ int b200seg_mscale_lo_bwd(const b200seg_mscale_desc* d, const void* g_lo, const 
 /* pr_pool / la_pool: fp32 [n][h/4+1][w/4+1][20] = avg_pool2d(sigmoid(joint)*mask + 1e-6) / avg_pool2d(onehot*mask) */
 int b200seg_rmi_pool(const b200seg_mscale_desc* d, const int64_t* labels, const float* hi_cls, const float* mid,
                      float* pr_pool, float* la_pool, void* stream);
+/* pr_pool of the auxiliary head (nheads 2, cfg.LOSS.OCR_AUX_RMI): the same pooling of sigmoid(joint_aux), where
+ * joint_aux blends mid channels 19..37 with up4(hi_aux) exactly as b200seg_rmi_pool blends head 0. The label pool is
+ * the one b200seg_rmi_pool wrote for head 0. */
+int b200seg_rmi_pool_aux(const b200seg_mscale_desc* d, const int64_t* labels, const float* hi_aux, const float* mid,
+                         float* pr_pool, void* stream);
 size_t b200seg_rmi_ws_bytes(int32_t n);
 /* Second moments (fp64) -> per (image, class) 9x9 Cholesky solves -> rmi_terms[n*19] (each already multiplied by
  * scale = w_head0 * (1 - lambda) / (n * 9)) and dpr = d(sum rmi_terms) / d pr_pool, fp32 [n][h/4+1][w/4+1][20].

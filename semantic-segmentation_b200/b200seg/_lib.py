@@ -127,12 +127,16 @@ SIGNATURES = {
     "b200seg_bias_grad": (ctypes.c_int, [V, I32, I64, I32, V, V]),
     "b200seg_count_valid": (ctypes.c_int, [V, I64, I32, I32, V, V, V]),
     "b200seg_rmi_pool": (ctypes.c_int, [ctypes.POINTER(MscaleDesc), V, V, V, V, V, V]),
+    "b200seg_rmi_pool_aux": (ctypes.c_int, [ctypes.POINTER(MscaleDesc), V, V, V, V, V]),
     "b200seg_rmi_ws_bytes": (c_size_t, [I32]),
     "b200seg_rmi_solve_grad": (ctypes.c_int, [I32, I32, I32, V, V, F, V, c_size_t, V, V, V, V]),
     "b200seg_mscale_mid_fwd": (ctypes.c_int, [ctypes.POINTER(MscaleDesc), V, V, V, V, V, V]),
     "b200seg_mscale_loss_blocks": (I32, [ctypes.POINTER(MscaleDesc)]),
     "b200seg_mscale_loss_fwd": (ctypes.c_int, [ctypes.POINTER(MscaleDesc), V, V, V, V, V, V, V, V, V, V, V, V, V, I32,
                                                V]),
+    "b200seg_mscale_loss_fwd_ex": (ctypes.c_int, [ctypes.POINTER(MscaleDesc), V, V, V, V, V, V, V, V, V, V, V, V, V,
+                                                  V, I32, V, V, I32, V]),
+    "b200seg_label_class_weights": (ctypes.c_int, [V, I32, I64, F, I32, V, V, V, V, V]),
     "b200seg_mscale_hi_bwd": (ctypes.c_int, [ctypes.POINTER(MscaleDesc), V, V, V, V]),
     "b200seg_mscale_lo_bwd": (ctypes.c_int, [ctypes.POINTER(MscaleDesc), V, V, V, V, V, V, V, V, V, V, V]),
     "b200seg_resize_to_nchw": (ctypes.c_int, [V, I32, I32, I32, I32, I32, I32, V, I32, I32, V]),

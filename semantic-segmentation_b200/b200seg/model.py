@@ -312,14 +312,16 @@ def scale_pass(E, images, size_hw, arch, hcfg, ocfg):
 
 
 def train_loss(E, images, gts, arch, hcfg, ocfg, lo_scale=0.5, ocr_alpha=0.4, sup_wt=0.0, ignore_index=255, E_lo=None,
-               loss_kind="ce"):
+               loss_kind="ce", img_wt=(1.0, False), ocr_aux_rmi=False):
     """Training forward + loss. ocrnet.HRNet_Mscale: MscaleOCR.two_scale_forward (network/ocrnet.py:264-319);
     mscale.HRNet: MscaleBase.two_scale_forward (network/mscale.py:182-220; one head, no auxiliary loss);
     ocrnet.HRNet: OCRNet.forward (:104-122); basic.HRNet: Basic.forward (network/basic.py:50-64).
-    Returns the fp32 loss vector [total, cls, aux, sup_lo, sup_hi, rmi, 0, 0]; pushes the loss backward on the tape.
-    loss_kind "ce": CrossEntropyLoss2d (loss/utils.py:133-134); "rmi": RMILoss (loss/rmi.py:70-215) = sigmoid BCE on
-    every head (the auxiliary / supervised terms are called with do_rmi=False, network/ocrnet.py:303-318) plus the
-    region-mutual-information term on the main prediction.
+    Returns the fp32 loss vector [total, cls, aux, sup_lo, sup_hi, rmi, aux rmi, 0]; pushes the loss backward on the
+    tape. loss_kind "ce": CrossEntropyLoss2d (loss/utils.py:133-134); "rmi": RMILoss (loss/rmi.py:70-215) = sigmoid BCE
+    on every head (the auxiliary / supervised terms are called with do_rmi=False, network/ocrnet.py:303-318) plus the
+    region-mutual-information term on the main prediction; ocr_aux_rmi (cfg.LOSS.OCR_AUX_RMI) calls the auxiliary head
+    with do_rmi=True as well. "img_wt": ImageBasedCrossEntropyLoss2d (loss/utils.py:70-118) with
+    img_wt = (upper_bound, round the weights through binary16), on every head and supervised term.
 
     E_lo (optional, two-scale only): a second engine with its own stream, gradient buffer and BN batch-statistics
     slots. The 0.5x and 1.0x passes are independent until the blend, so the low-resolution program is enqueued on
@@ -359,12 +361,22 @@ def train_loss(E, images, gts, arch, hcfg, ocfg, lo_scale=0.5, ocr_alpha=0.4, su
     else:
         d = raw.mscale_desc(n, H, W, hq, wq, 0, 0, 0, 0, nheads, 1.0, ocr_alpha, 0.0, ignore_index, kind)
         mid = mid_sup = None
-    inv_count = raw.count_valid(gts, ignore_index, plus_one=rmi)
-    dpr = terms = None
+    coef = None
+    if loss_kind == "img_wt":
+        # one histogram of the whole local batch per step; every head reads the same per-image coefficients
+        _, _, coef, inv_count = raw.label_class_weights(gts, img_wt[0], img_wt[1])
+    else:
+        inv_count = raw.count_valid(gts, ignore_index, plus_one=rmi)
+    dpr = terms = dpr_aux = terms_aux = None
     if rmi:
-        dpr, terms = raw.rmi_head(d, gts, hi["cls"].logits, mid)
+        pr, la = raw.rmi_pool(d, gts, hi["cls"].logits, mid)
+        dpr, terms = raw.rmi_solve_grad(d, pr, la, d.w_head0)
+        if ocr_aux_rmi and nheads > 1:
+            pr_aux = raw.rmi_pool_aux(d, gts, hi["aux"].logits, mid)
+            dpr_aux, terms_aux = raw.rmi_solve_grad(d, pr_aux, la, d.w_head1)
     loss, g_hi, g_lo, g_sup = raw.mscale_loss_fwd(d, gts, inv_count, hi["cls"].logits,
-                                                  hi["aux"].logits if nheads > 1 else None, mid, mid_sup, dpr, terms)
+                                                  hi["aux"].logits if nheads > 1 else None, mid, mid_sup, dpr, terms,
+                                                  coef, dpr_aux, terms_aux)
 
     def loss_bwd():
         d_cls, d_aux = raw.mscale_hi_bwd(d, g_hi)

@@ -30,15 +30,41 @@ def _criterion_kind(criterion):
     if criterion is None:
         return "ce"
     if isinstance(criterion, str):
-        if criterion in ("ce", "rmi"):
-            return criterion
-        raise NotImplementedError("criterion %r: expected 'ce' or 'rmi'" % criterion)
+        if criterion in ("ce", "rmi") or criterion.split(":")[0] == "img_wt":
+            return criterion.split(":")[0]
+        raise NotImplementedError("criterion %r: expected 'ce', 'rmi' or 'img_wt[:upper_bound[:half]]'" % criterion)
     name = type(criterion).__name__
     if name in ("CrossEntropyLoss2d", "CrossEntropyLoss"):
         return "ce"
     if name == "RMILoss":
         return "rmi"
-    raise NotImplementedError("criterion %s is outside the B200 hot path (CE and RMI are covered)" % name)
+    if name == "ImageBasedCrossEntropyLoss2d":
+        return "img_wt"
+    if name == "ImgWtLossSoftNLL":
+        raise NotImplementedError(
+            "criterion ImgWtLossSoftNLL (--jointwtborder) is not covered: it needs the multi-hot border targets of the "
+            "dataset, and its forward(inputs, target) takes no do_rmi, so the reference itself raises a TypeError with "
+            "these architectures")
+    raise NotImplementedError("criterion %s is outside the B200 hot path (CE, RMI and image-weighted CE are covered)"
+                              % name)
+
+
+def _img_wt_options(criterion, ignore_index=255):
+    """ImageBasedCrossEntropyLoss2d (loss/utils.py:70-118) -> (upper_bound, round the weights through binary16).
+    The weights are rounded when cfg.BATCH_WEIGHTING is off and fp16 is on (weights.half(), read back as fp32 by
+    apex's nll_loss). String form: 'img_wt[:upper_bound[:half]]'."""
+    if isinstance(criterion, str):
+        parts = criterion.split(":")
+        return (float(parts[1]) if len(parts) > 1 else 1.0), (len(parts) > 2 and parts[2] == "half")
+    if getattr(criterion, "norm", False):
+        raise NotImplementedError("ImageBasedCrossEntropyLoss2d(norm=True) is not covered (get_loss never sets it)")
+    if getattr(criterion, "num_classes", 19) != 19:
+        raise NotImplementedError("ImageBasedCrossEntropyLoss2d: the class weights are instantiated for 19 classes")
+    crit_ignore = getattr(getattr(criterion, "nll_loss", None), "ignore_index", ignore_index)
+    if crit_ignore != ignore_index:
+        raise NotImplementedError("ImageBasedCrossEntropyLoss2d: ignore_index %d differs from the model's %d"
+                                  % (crit_ignore, ignore_index))
+    return float(criterion.upper_bound), bool(criterion.fp16) and not bool(criterion.batch_weights)
 
 
 def allreduce_sum_(flat):
@@ -81,11 +107,15 @@ class _PublishGrads(torch.autograd.Function):
 class B200SegModule(nn.Module):
     def __init__(self, arch, num_classes=19, criterion=None, hcfg=None, ocfg=None, lo_scale=0.5, ocr_alpha=0.4,
                  supervised_mscale_wt=0.0, ignore_index=255, n_scales=None, use_cuda_graph=True,
-                 parallel_scales=True, syncbn=None, parallel_branches=True):
+                 parallel_scales=True, syncbn=None, parallel_branches=True, ocr_aux_rmi=False):
         super().__init__()
         self.arch = arch
         self.criterion = criterion
         self.loss_kind = _criterion_kind(criterion)
+        self.img_wt = _img_wt_options(criterion, ignore_index) if self.loss_kind == "img_wt" else (1.0, False)
+        # cfg.LOSS.OCR_AUX_RMI: the auxiliary head is called with do_rmi=True (network/ocrnet.py:116,302-303); only the
+        # RMILoss criterion reads do_rmi, and only the OCR architectures have an auxiliary head
+        self.ocr_aux_rmi = bool(ocr_aux_rmi)
         self.is_deepv3 = arch == "deepv3.DeepV3PlusW38"
         self.hcfg = hcfg or (A.WRN38 if self.is_deepv3 else A.HRNET_W48)
         self._stem = "backbone.mod1.conv1.weight" if self.is_deepv3 else "backbone.conv1.weight"
@@ -464,7 +494,8 @@ class B200SegModule(nn.Module):
                    bnfold=self._bnfold[1] if self.fused_bn_finalize else None,
                    bncells=self._bncells[1] if use_cells else None)
         loss = M.train_loss(E, images, gts, self.arch, self.hcfg, self.ocfg, self.lo_scale, self.ocr_alpha, self.sup_wt,
-                            self.ignore_index, E_lo=E_lo, loss_kind=self.loss_kind)
+                            self.ignore_index, E_lo=E_lo, loss_kind=self.loss_kind, img_wt=self.img_wt,
+                            ocr_aux_rmi=self.ocr_aux_rmi)
         E.pre_backward_event = wd_ready
         if E_lo is not None:
             E_lo.pre_backward_event = wd_ready

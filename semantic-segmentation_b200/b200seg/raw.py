@@ -529,24 +529,59 @@ def count_valid(labels, ignore_index=255, plus_one=False):
     return inv
 
 
-def rmi_head(d, labels, hi_cls, mid):
-    """RMI term of head 0 (loss/rmi.py rmi_lower_bound): -> (dpr fp32 [n,h/4+1,w/4+1,20], rmi_terms fp32 [n*19])."""
+def rmi_pool(d, labels, hi_cls, mid):
+    """-> (pr_pool, la_pool) fp32 [n,h/4+1,w/4+1,20] of head 0 (avg-pooled sigmoid probabilities and one-hot labels)."""
     dev = hi_cls.device
-    n, hp, wp = d.n, d.h // 4 + 1, d.w // 4 + 1
-    L = lib()
-    pr = _new((n, hp, wp, 20), dtype=F32, device=dev)
-    la = _new((n, hp, wp, 20), dtype=F32, device=dev)
-    check(L.b200seg_rmi_pool(ctypes.byref(d), ptr(labels), ptr(hi_cls), ptr(mid), ptr(pr), ptr(la), stream_ptr()),
+    pr = _new((d.n, d.h // 4 + 1, d.w // 4 + 1, 20), dtype=F32, device=dev)
+    la = _new((d.n, d.h // 4 + 1, d.w // 4 + 1, 20), dtype=F32, device=dev)
+    check(lib().b200seg_rmi_pool(ctypes.byref(d), ptr(labels), ptr(hi_cls), ptr(mid), ptr(pr), ptr(la), stream_ptr()),
           "rmi_pool")
+    return pr, la
+
+
+def rmi_pool_aux(d, labels, hi_aux, mid):
+    """-> pr_pool of the auxiliary head (cfg.LOSS.OCR_AUX_RMI); its label pool is head 0's."""
+    pr = _new((d.n, d.h // 4 + 1, d.w // 4 + 1, 20), dtype=F32, device=hi_aux.device)
+    check(lib().b200seg_rmi_pool_aux(ctypes.byref(d), ptr(labels), ptr(hi_aux), ptr(mid), ptr(pr), stream_ptr()),
+          "rmi_pool_aux")
+    return pr
+
+
+def rmi_solve_grad(d, pr, la, head_weight):
+    """RMI term of one head with loss weight head_weight: -> (dpr fp32 [n,h/4+1,w/4+1,20], rmi_terms fp32 [n*19])."""
+    dev = pr.device
+    n = d.n
+    L = lib()
     nbytes = L.b200seg_rmi_ws_bytes(n)
     ws = _new((nbytes // 8,), dtype=torch.float64, device=dev)
     G = _new((n, 19, 180), dtype=torch.float64, device=dev)
     terms = _new((n * 19,), dtype=F32, device=dev)
-    dpr = _new((n, hp, wp, 20), dtype=F32, device=dev)
-    scale = d.w_head0 * (1.0 - RMI_LAMBDA) / (n * 9.0)
+    dpr = _new(tuple(pr.shape), dtype=F32, device=dev)
+    scale = head_weight * (1.0 - RMI_LAMBDA) / (n * 9.0)
     check(L.b200seg_rmi_solve_grad(n, d.h, d.w, ptr(pr), ptr(la), scale, ptr(ws), nbytes, ptr(G), ptr(terms), ptr(dpr),
                                    stream_ptr()), "rmi_solve_grad", 3)
     return dpr, terms
+
+
+def rmi_head(d, labels, hi_cls, mid):
+    """RMI term of head 0 (loss/rmi.py rmi_lower_bound): -> (dpr fp32 [n,h/4+1,w/4+1,20], rmi_terms fp32 [n*19])."""
+    pr, la = rmi_pool(d, labels, hi_cls, mid)
+    return rmi_solve_grad(d, pr, la, d.w_head0)
+
+
+def label_class_weights(labels, upper_bound, round_half=False):
+    """ImageBasedCrossEntropyLoss2d.calculate_weights on the whole batch (loss/utils.py:86-99) -> (counts int32 [n,19],
+    weights fp32 [19], coef fp32 [n,19] = w[c] / sum_c w[c] counts[i][c], loss_scale fp32 [1] = 1 or NaN)."""
+    n = labels.shape[0]
+    dev = labels.device
+    counts = _new((n, 19), dtype=torch.int32, device=dev)
+    weights = _new((19,), dtype=F32, device=dev)
+    coef = _new((n, 19), dtype=F32, device=dev)
+    scale = _new((1,), dtype=F32, device=dev)
+    check(lib().b200seg_label_class_weights(ptr(labels), n, labels.numel() // n, float(upper_bound), int(round_half),
+                                            ptr(counts), ptr(weights), ptr(coef), ptr(scale), stream_ptr()),
+          "label_class_weights", 2)
+    return counts, weights, coef, scale
 
 
 def mscale_mid_fwd(d, lo_cls, lo_aux, lo_attn):
@@ -558,7 +593,10 @@ def mscale_mid_fwd(d, lo_cls, lo_aux, lo_attn):
     return mid, mid_sup
 
 
-def mscale_loss_fwd(d, labels, inv_count, hi_cls, hi_aux, mid, mid_sup, rmi_dpr=None, rmi_terms=None):
+def mscale_loss_fwd(d, labels, inv_count, hi_cls, hi_aux, mid, mid_sup, rmi_dpr=None, rmi_terms=None, class_coef=None,
+                    rmi_dpr_aux=None, rmi_terms_aux=None):
+    """class_coef: image-weighted CE (inv_count = the loss_scale of label_class_weights); rmi_dpr_aux / rmi_terms_aux:
+    RMI on the auxiliary head (cfg.LOSS.OCR_AUX_RMI)."""
     dev = hi_cls.device
     L = lib()
     nb = L.b200seg_mscale_loss_blocks(ctypes.byref(d))
@@ -567,11 +605,19 @@ def mscale_loss_fwd(d, labels, inv_count, hi_cls, hi_aux, mid, mid_sup, rmi_dpr=
     g_lo = _new((npix, 40), dtype=BF16, device=dev) if d.hm > 0 else None
     g_sup = _new((npix, 40), dtype=BF16, device=dev) if (d.hm > 0 and d.sup_wt != 0.0) else None
     ws = _new((nb * 4,), dtype=F32, device=dev)
-    loss = _newz((8,), dtype=F32, device=dev)   # total, 4 pointwise means, RMI term, 2 pad
-    check(L.b200seg_mscale_loss_fwd(ctypes.byref(d), ptr(labels), ptr(inv_count), ptr(hi_cls), ptr(hi_aux), ptr(mid),
-                                    ptr(mid_sup), ptr(g_hi), ptr(g_lo), ptr(g_sup), ptr(ws), ptr(loss), ptr(rmi_dpr),
-                                    ptr(rmi_terms), rmi_terms.numel() if rmi_terms is not None else 0, stream_ptr()),
-          "mscale_loss_fwd", 2)
+    loss = _newz((8,), dtype=F32, device=dev)   # total, 4 pointwise means, RMI term, auxiliary RMI term, pad
+    n_terms = rmi_terms.numel() if rmi_terms is not None else 0
+    if class_coef is None and rmi_dpr_aux is None:
+        rc = L.b200seg_mscale_loss_fwd(ctypes.byref(d), ptr(labels), ptr(inv_count), ptr(hi_cls), ptr(hi_aux), ptr(mid),
+                                       ptr(mid_sup), ptr(g_hi), ptr(g_lo), ptr(g_sup), ptr(ws), ptr(loss), ptr(rmi_dpr),
+                                       ptr(rmi_terms), n_terms, stream_ptr())
+    else:
+        rc = L.b200seg_mscale_loss_fwd_ex(ctypes.byref(d), ptr(labels), ptr(inv_count), ptr(class_coef), ptr(hi_cls),
+                                          ptr(hi_aux), ptr(mid), ptr(mid_sup), ptr(g_hi), ptr(g_lo), ptr(g_sup), ptr(ws),
+                                          ptr(loss), ptr(rmi_dpr), ptr(rmi_terms), n_terms, ptr(rmi_dpr_aux),
+                                          ptr(rmi_terms_aux), rmi_terms_aux.numel() if rmi_terms_aux is not None else 0,
+                                          stream_ptr())
+    check(rc, "mscale_loss_fwd", 2)
     return loss, g_hi, g_lo, g_sup
 
 

@@ -76,20 +76,23 @@ struct MsGeom {
   int loss_kind;      // 0: softmax cross-entropy heads; 1: RMILoss criterion (sigmoid BCE heads + RMI on head 0)
 };
 
-// Blended class logits of head 0 at full-resolution pixel (n, Y, X): joint = up2(attn*cls_lo) + (1 - up2(attn)) * up4(cls_hi)
-// (network/ocrnet.py:289-298); without a lo pass just up4(cls_hi). Same association order as the loss kernel.
-__device__ __forceinline__ void joint_head0(const MsGeom& g, int n, int Y, int X, const float* __restrict__ hi_cls,
-                                            const float* __restrict__ M, float (&J)[NC]) {
+// Blended logits of head kHead (0: cls, 1: aux) at full-resolution pixel (n, Y, X):
+// joint = up2(attn*lo) + (1 - up2(attn)) * up4(hi) (network/ocrnet.py:289-298); without a lo pass just up4(hi).
+// hi: that head's quarter-resolution map; the head's blended lo part sits in mid channels [kHead*19, kHead*19+19).
+// Same association order as the loss kernel.
+template <int kHead>
+__device__ __forceinline__ void joint_head(const MsGeom& g, int n, int Y, int X, const float* __restrict__ hi,
+                                           const float* __restrict__ M, float (&J)[NC]) {
   const TapW th = make_tapw(Y, X, g.H, g.W, g.Hq, g.Wq);
   const size_t imq = (size_t)n * g.Hq * g.Wq;
 #pragma unroll
-  for (int c = 0; c < NC; ++c) J[c] = interp(th, hi_cls + imq * LD, g.Wq, LD, c);
+  for (int c = 0; c < NC; ++c) J[c] = interp(th, hi + imq * LD, g.Wq, LD, c);
   if (g.Hm > 0) {
     const TapW tm = make_tapw(Y, X, g.H, g.W, g.Hm, g.Wm);
     const size_t imm = (size_t)n * g.Hm * g.Wm;
     const float oma = 1.f - interp(tm, M + imm * MW, g.Wm, MW, 2 * NC);
 #pragma unroll
-    for (int c = 0; c < NC; ++c) J[c] = interp(tm, M + imm * MW, g.Wm, MW, c) + oma * J[c];
+    for (int c = 0; c < NC; ++c) J[c] = interp(tm, M + imm * MW, g.Wm, MW, kHead * NC + c) + oma * J[c];
   }
 }
 

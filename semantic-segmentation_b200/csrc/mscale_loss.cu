@@ -16,6 +16,10 @@
 //   hi_bwd       adjoint of the x4 upsample: Ghi -> d cls_hi, d aux_hi
 //   mid_bwd      adjoint of the x2 upsample + product rule at the mid grid -> D[m][40]
 //   lo_bwd       adjoint of the x4 upsample on the lo pass -> d cls_lo, d aux_lo, d attn_logit (through the sigmoid)
+//   label_hist / class_weights   per-image class counts and the class weights of ImageBasedCrossEntropyLoss2d, read by
+//                the weighted instantiation of loss_fwd
+#include <cuda_fp16.h>
+#include <algorithm>
 #include "ptx.cuh"
 #include "launch.h"
 #include "../../include/b200seg.h"
@@ -114,17 +118,24 @@ __device__ __forceinline__ void store_row40(__nv_bfloat16* dst, const float (&a)
 
 // ------------------------------------------------------------------------------------------------ loss_fwd
 // partial[block][4] = sums of nll over valid pixels for {cls head, aux head, supervised lo, supervised hi}
+// kWt (ImageBasedCrossEntropyLoss2d, loss/utils.py:70-118): every pixel's nll and gradient are scaled by
+//   class_coef[n][label] = w[label] / sum_p w[y_p] over the valid pixels of image n, so the partial sums already hold the
+//   sum over images of the per-image weighted means; inv_count then only carries the NaN of an image without a valid pixel
+//   into the loss (the gradient must not see it).
+// kAuxRmi (cfg.LOSS.OCR_AUX_RMI, network/ocrnet.py:116,302-303): head 1 is called with do_rmi=True like head 0: lambda * BCE
+//   plus the RMI gradient rmi_dpr_aux of its own pooled probabilities.
+template <bool kWt, bool kAuxRmi>
 __global__ void __launch_bounds__(128)
 loss_fwd_kernel(const MsGeom g, const long long* __restrict__ labels, const float* __restrict__ inv_count,
                 const float* __restrict__ hi_cls, const float* __restrict__ hi_aux, const float* __restrict__ M,
                 const float* __restrict__ M2, __nv_bfloat16* __restrict__ Ghi, __nv_bfloat16* __restrict__ Glo,
                 __nv_bfloat16* __restrict__ Gsup, float* __restrict__ partial, const float* __restrict__ rmi_dpr,
-                int Hp, int Wp) {
+                int Hp, int Wp, const float* __restrict__ class_coef, const float* __restrict__ rmi_dpr_aux) {
   pdl_sync();
   const long long total = (long long)g.N * g.H * g.W;
   const bool has_lo = g.Hm > 0;
   const bool rmi = g.loss_kind == 1;
-  const float icnt = *inv_count;
+  const float icnt = kWt ? 1.f : *inv_count;
   float acc[4] = {0.f, 0.f, 0.f, 0.f};
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
        idx += (long long)gridDim.x * blockDim.x) {
@@ -132,6 +143,9 @@ loss_fwd_kernel(const MsGeom g, const long long* __restrict__ labels, const floa
     const long long lab64 = labels[idx];
     const bool valid = lab64 != (long long)g.ignore_index;
     const int label = valid ? (int)lab64 : -1;
+    float pw = 1.f;
+    if constexpr (kWt) pw = (valid && (unsigned)label < (unsigned)NC) ? class_coef[(size_t)n * NC + label] : 0.f;
+    const auto wt = [pw](float x) { return kWt ? x * pw : x; };
     const TapW th = make_tapw(Y, X, g.H, g.W, g.Hq, g.Wq);
     const size_t imq = (size_t)n * g.Hq * g.Wq;
     float hc[NC], ha[NC];
@@ -173,10 +187,21 @@ loss_fwd_kernel(const MsGeom g, const long long* __restrict__ labels, const floa
 #pragma unroll
         for (int c = 0; c < NC; ++c) Jc[c] += dp[c] * 0.0625f * P[c] * (1.f - P[c]);
       }
-      if (g.nheads > 1) acc[1] += bce_grad(Ja, label, valid, g.w_head1 * icnt, nullptr);   // aux head: do_rmi=False
+      if (g.nheads > 1) {
+        if constexpr (kAuxRmi) {
+          acc[1] += bce_grad(Ja, label, valid, g.w_head1 * kRmiLambda * icnt, P);
+          if (valid) {
+            const float* dp = rmi_dpr_aux + (((size_t)n * Hp + ((Y + 2) >> 2)) * Wp + ((X + 2) >> 2)) * LD;
+#pragma unroll
+            for (int c = 0; c < NC; ++c) Ja[c] += dp[c] * 0.0625f * P[c] * (1.f - P[c]);
+          }
+        } else {
+          acc[1] += bce_grad(Ja, label, valid, g.w_head1 * icnt, nullptr);   // aux head: do_rmi=False
+        }
+      }
     } else {
-      acc[0] += ce_grad(Jc, label, valid, g.w_head0 * icnt);
-      if (g.nheads > 1) acc[1] += ce_grad(Ja, label, valid, g.w_head1 * icnt);
+      acc[0] += wt(ce_grad(Jc, label, valid, wt(g.w_head0 * icnt)));
+      if (g.nheads > 1) acc[1] += wt(ce_grad(Ja, label, valid, wt(g.w_head1 * icnt)));
     }
     if (g.nheads <= 1) {
 #pragma unroll
@@ -197,13 +222,15 @@ loss_fwd_kernel(const MsGeom g, const long long* __restrict__ labels, const floa
       float S[NC];
 #pragma unroll
       for (int c = 0; c < NC; ++c) S[c] = hc[c];
-      acc[3] += rmi ? bce_grad(S, label, valid, g.sup_wt * icnt, nullptr) : ce_grad(S, label, valid, g.sup_wt * icnt);
+      acc[3] += rmi ? bce_grad(S, label, valid, g.sup_wt * icnt, nullptr)
+                    : wt(ce_grad(S, label, valid, wt(g.sup_wt * icnt)));
 #pragma unroll
       for (int c = 0; c < NC; ++c) gh[c] += S[c];
       if (has_lo) {
 #pragma unroll
         for (int c = 0; c < NC; ++c) S[c] = interp(tm, M2 + imm * LD, g.Wm, LD, c);
-        acc[2] += rmi ? bce_grad(S, label, valid, g.sup_wt * icnt, nullptr) : ce_grad(S, label, valid, g.sup_wt * icnt);
+        acc[2] += rmi ? bce_grad(S, label, valid, g.sup_wt * icnt, nullptr)
+                      : wt(ce_grad(S, label, valid, wt(g.sup_wt * icnt)));
         float z[NC];
 #pragma unroll
         for (int c = 0; c < NC; ++c) z[c] = 0.f;
@@ -227,10 +254,12 @@ loss_fwd_kernel(const MsGeom g, const long long* __restrict__ labels, const floa
         (s_acc[0][threadIdx.x] + s_acc[1][threadIdx.x]) + (s_acc[2][threadIdx.x] + s_acc[3][threadIdx.x]);
 }
 
-// loss = icnt * (w0*s0 + w1*s1 + sup*(s2 + s3)); also returns the four mean NLLs
+// loss = icnt * (w0*s0 + w1*s1 + sup*(s2 + s3)) + RMI terms of head 0 (out[5]) and of head 1 (out[6]); also returns the
+// four mean NLLs
 __global__ void loss_finalize_kernel(const float* __restrict__ partial, int nblocks, const float* __restrict__ inv_count,
                                      float w0, float w1, float sup, float* __restrict__ out,
-                                     const float* __restrict__ rmi_terms, int n_rmi) {
+                                     const float* __restrict__ rmi_terms, int n_rmi,
+                                     const float* __restrict__ rmi_terms_aux, int n_rmi_aux) {
   pdl_sync();
   __shared__ double s[4][32];
   double a[4] = {0, 0, 0, 0};
@@ -245,10 +274,78 @@ __global__ void loss_finalize_kernel(const float* __restrict__ partial, int nblo
     const double ic = (double)*inv_count;
     double r = 0.0;                          // (1 - lambda) * w0 * sum_c mean_n(rmi_nc) / 9, already scaled per term
     for (int i = 0; i < n_rmi; ++i) r += (double)rmi_terms[i];
-    out[0] = (float)(ic * (w0 * t[0] + w1 * t[1] + sup * (t[2] + t[3])) + r);
+    double ra = 0.0;
+    for (int i = 0; i < n_rmi_aux; ++i) ra += (double)rmi_terms_aux[i];
+    out[0] = (float)(ic * (w0 * t[0] + w1 * t[1] + sup * (t[2] + t[3])) + (r + ra));
     for (int k = 0; k < 4; ++k) out[1 + k] = (float)(ic * t[k]);
     out[5] = (float)r;
+    out[6] = (float)ra;
   }
+}
+
+// ------------------------------------------------------------------------------------------------ image-weighted CE
+// ImageBasedCrossEntropyLoss2d.calculate_weights (loss/utils.py:86-99): per-image class counts of the labels in [0, 19)
+// (ignore_index 255 falls outside histc's range). Shared-memory block histogram, one leader atomic per distinct label of
+// a warp; integer sums, so the counts do not depend on the schedule. grid (blocks, n); counts zeroed by the caller.
+__global__ void __launch_bounds__(256)
+label_hist_kernel(const long long* __restrict__ labels, long long per_image, int* __restrict__ counts) {
+  pdl_sync();
+  __shared__ int h[NC];
+  if (threadIdx.x < NC) h[threadIdx.x] = 0;
+  __syncthreads();
+  const long long* lab = labels + (size_t)blockIdx.y * per_image;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long base = (long long)blockIdx.x * blockDim.x; base < per_image; base += stride) {   // warp-uniform trip
+    const long long i = base + threadIdx.x;
+    const long long v = i < per_image ? lab[i] : -1;
+    const int bin = (v >= 0 && v < NC) ? (int)v : -1;
+    const unsigned peers = __match_any_sync(0xffffffffu, bin);
+    if (bin >= 0 && (threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&h[bin], __popc(peers));
+  }
+  __syncthreads();
+  if (threadIdx.x < NC && h[threadIdx.x]) atomicAdd(&counts[(size_t)blockIdx.y * NC + threadIdx.x], h[threadIdx.x]);
+}
+
+// One block of 32 threads. Batch bins b[c] = sum_n counts[n][c]; w[c] = (b[c] != 0) * ub * (1 - b[c] / sum b) + 1 in
+// separate fp32 operations in PyTorch's order (no contraction), optionally rounded through binary16 (weights.half() when
+// cfg.BATCH_WEIGHTING is off under fp16; apex's nll_loss reads them back as fp32). coef[n][c] = w[c] / sum_c w[c] count[n][c]
+// (fp64 denominator): the weight nll_loss(reduction='mean') gives a pixel of class c in image n. An image without a valid
+// pixel gets a NaN row and sets loss_scale to NaN (the reference's 0/0), otherwise loss_scale = 1.
+__global__ void __launch_bounds__(32)
+class_weights_kernel(const int* __restrict__ counts, int n, float upper_bound, int round_half, float* __restrict__ weights,
+                     float* __restrict__ coef, float* __restrict__ loss_scale) {
+  pdl_sync();
+  __shared__ long long s_bins[NC];
+  __shared__ float s_w[NC];
+  __shared__ int s_empty;
+  const int c = threadIdx.x;
+  if (c == 0) s_empty = 0;
+  if (c < NC) {
+    long long b = 0;
+    for (int i = 0; i < n; ++i) b += counts[(size_t)i * NC + c];
+    s_bins[c] = b;
+  }
+  __syncthreads();
+  if (c < NC) {
+    long long total = 0;
+    for (int k = 0; k < NC; ++k) total += s_bins[k];
+    const float hist_norm = __fdiv_rn((float)s_bins[c], (float)total);
+    const float nz = s_bins[c] != 0 ? 1.f : 0.f;
+    float w = __fadd_rn(__fmul_rn(__fmul_rn(nz, upper_bound), __fsub_rn(1.f, hist_norm)), 1.f);
+    if (round_half) w = __half2float(__float2half_rn(w));
+    s_w[c] = w;
+    weights[c] = w;
+  }
+  __syncthreads();
+  for (int i = c; i < n; i += blockDim.x) {
+    double den = 0.0;
+    for (int k = 0; k < NC; ++k) den += (double)s_w[k] * (double)counts[(size_t)i * NC + k];
+    if (den == 0.0) s_empty = 1;
+    for (int k = 0; k < NC; ++k)
+      coef[(size_t)i * NC + k] = den == 0.0 ? __int_as_float(0x7fc00000) : (float)((double)s_w[k] / den);
+  }
+  __syncthreads();
+  if (c == 0) *loss_scale = s_empty ? __int_as_float(0x7fc00000) : 1.f;
 }
 
 __global__ void count_valid_kernel(const long long* __restrict__ labels, long long total, int ignore_index,
@@ -503,26 +600,66 @@ extern "C" int b200seg_mscale_mid_fwd(const b200seg_mscale_desc* d, const float*
   RET_LAUNCH();
 }
 
-extern "C" int b200seg_mscale_loss_fwd(const b200seg_mscale_desc* d, const int64_t* labels, const float* inv_count,
-                                       const float* hi_cls, const float* hi_aux, const float* mid, const float* mid_sup,
-                                       void* g_hi, void* g_lo, void* g_sup, float* partial_ws, float* loss_out,
-                                       const float* rmi_dpr, const float* rmi_terms, int32_t n_rmi_terms,
-                                       void* stream) {
+extern "C" int b200seg_label_class_weights(const int64_t* labels, int32_t n, int64_t per_image, float upper_bound,
+                                           int32_t round_half, int32_t* counts, float* weights, float* coef,
+                                           float* loss_scale, void* stream) {
+  if (!labels || n <= 0 || per_image <= 0 || !counts || !weights || !coef || !loss_scale) return B200SEG_E_BADARG;
+  cudaError_t e = cudaMemsetAsync(counts, 0, (size_t)n * NC * sizeof(int32_t), (cudaStream_t)stream);
+  if (e != cudaSuccess) return (int)e;
+  const long long bx = std::max(1LL, std::min<long long>((per_image + 2047) / 2048, 132LL * 4 / n));
+  launch_k(label_hist_kernel, dim3((unsigned)bx, n), dim3(256), 0, (cudaStream_t)stream, (const long long*)labels,
+           (long long)per_image, (int*)counts);
+  launch_k(class_weights_kernel, dim3(1), dim3(32), 0, (cudaStream_t)stream, (const int*)counts, (int)n, upper_bound,
+           (int)round_half, weights, coef, loss_scale);
+  RET_LAUNCH();
+}
+
+static int loss_fwd_launch(const b200seg_mscale_desc* d, const int64_t* labels, const float* inv_count,
+                           const float* class_coef, const float* hi_cls, const float* hi_aux, const float* mid,
+                           const float* mid_sup, void* g_hi, void* g_lo, void* g_sup, float* partial_ws,
+                           float* loss_out, const float* rmi_dpr, const float* rmi_terms, int32_t n_rmi_terms,
+                           const float* rmi_dpr_aux, const float* rmi_terms_aux, int32_t n_rmi_terms_aux,
+                           void* stream) {
   if (!d || !labels || !inv_count || !hi_cls || !g_hi || !partial_ws || !loss_out) return B200SEG_E_BADARG;
   if (d->nheads > 1 && !hi_aux) return B200SEG_E_BADARG;
   if (d->hm > 0 && (!mid || !g_lo)) return B200SEG_E_BADARG;
   if (d->sup_wt != 0.f && d->hm > 0 && (!mid_sup || !g_sup)) return B200SEG_E_BADARG;
   if (d->loss_kind != 0 && d->loss_kind != 1) return B200SEG_E_BADARG;
   if (n_rmi_terms > 0 && !rmi_terms) return B200SEG_E_BADARG;
+  if (n_rmi_terms_aux > 0 && !rmi_terms_aux) return B200SEG_E_BADARG;
+  if (class_coef && d->loss_kind != 0) return B200SEG_E_BADARG;                    // the weighted criterion is CE
+  if (rmi_dpr_aux && (d->loss_kind != 1 || d->nheads < 2)) return B200SEG_E_BADARG;
   const int nb = b200seg_mscale_loss_blocks(d);
   const int Hp = d->h / 4 + 1, Wp = d->w / 4 + 1;     // avg_pool2d(kernel 4, stride 4, padding 2) output size
-  launch_k(loss_fwd_kernel, dim3(nb), dim3(128), 0, (cudaStream_t)stream, to_geom(d), (const long long*)labels,
-           inv_count, hi_cls, hi_aux, mid, mid_sup, (__nv_bfloat16*)g_hi, (__nv_bfloat16*)g_lo, (__nv_bfloat16*)g_sup,
-           partial_ws, rmi_dpr, Hp, Wp);
+  auto kern = class_coef ? loss_fwd_kernel<true, false>
+                         : (rmi_dpr_aux ? loss_fwd_kernel<false, true> : loss_fwd_kernel<false, false>);
+  launch_k(kern, dim3(nb), dim3(128), 0, (cudaStream_t)stream, to_geom(d), (const long long*)labels, inv_count, hi_cls,
+           hi_aux, mid, mid_sup, (__nv_bfloat16*)g_hi, (__nv_bfloat16*)g_lo, (__nv_bfloat16*)g_sup, partial_ws, rmi_dpr,
+           Hp, Wp, class_coef, rmi_dpr_aux);
+  const float w1 = d->nheads > 1 ? (rmi_dpr_aux ? d->w_head1 * kRmiLambda : d->w_head1) : 0.f;
   launch_k(loss_finalize_kernel, dim3(1), dim3(32), 0, (cudaStream_t)stream, partial_ws, nb, inv_count,
-           d->loss_kind == 1 ? d->w_head0 * kRmiLambda : d->w_head0, d->nheads > 1 ? d->w_head1 : 0.f, d->sup_wt,
-           loss_out, rmi_terms, (int)n_rmi_terms);
+           d->loss_kind == 1 ? d->w_head0 * kRmiLambda : d->w_head0, w1, d->sup_wt, loss_out, rmi_terms,
+           (int)n_rmi_terms, rmi_terms_aux, (int)n_rmi_terms_aux);
   RET_LAUNCH();
+}
+
+extern "C" int b200seg_mscale_loss_fwd(const b200seg_mscale_desc* d, const int64_t* labels, const float* inv_count,
+                                       const float* hi_cls, const float* hi_aux, const float* mid, const float* mid_sup,
+                                       void* g_hi, void* g_lo, void* g_sup, float* partial_ws, float* loss_out,
+                                       const float* rmi_dpr, const float* rmi_terms, int32_t n_rmi_terms,
+                                       void* stream) {
+  return loss_fwd_launch(d, labels, inv_count, nullptr, hi_cls, hi_aux, mid, mid_sup, g_hi, g_lo, g_sup, partial_ws,
+                         loss_out, rmi_dpr, rmi_terms, n_rmi_terms, nullptr, nullptr, 0, stream);
+}
+
+extern "C" int b200seg_mscale_loss_fwd_ex(const b200seg_mscale_desc* d, const int64_t* labels, const float* inv_count,
+                                          const float* class_coef, const float* hi_cls, const float* hi_aux,
+                                          const float* mid, const float* mid_sup, void* g_hi, void* g_lo, void* g_sup,
+                                          float* partial_ws, float* loss_out, const float* rmi_dpr,
+                                          const float* rmi_terms, int32_t n_rmi_terms, const float* rmi_dpr_aux,
+                                          const float* rmi_terms_aux, int32_t n_rmi_terms_aux, void* stream) {
+  return loss_fwd_launch(d, labels, inv_count, class_coef, hi_cls, hi_aux, mid, mid_sup, g_hi, g_lo, g_sup, partial_ws,
+                         loss_out, rmi_dpr, rmi_terms, n_rmi_terms, rmi_dpr_aux, rmi_terms_aux, n_rmi_terms_aux, stream);
 }
 
 extern "C" int b200seg_mscale_hi_bwd(const b200seg_mscale_desc* d, const void* g_hi, void* d_cls, void* d_aux,

@@ -30,6 +30,9 @@ constexpr int kGPitch = 180;         // doubles per (image, class) gradient reco
 constexpr float kClipMin = 1e-6f;
 constexpr double kPosAlpha = 5e-4;
 
+// kHead 0: the main prediction (pr_pool and la_pool); kHead 1: the auxiliary prediction under cfg.LOSS.OCR_AUX_RMI
+// (pr_pool only: the label pool is the same for both heads).
+template <int kHead>
 __global__ void __launch_bounds__(128)
 rmi_pool_kernel(const MsGeom g, const long long* __restrict__ labels, const float* __restrict__ hi_cls,
                 const float* __restrict__ M, float* __restrict__ pr_pool, float* __restrict__ la_pool, int Hp, int Wp) {
@@ -50,20 +53,24 @@ rmi_pool_kernel(const MsGeom g, const long long* __restrict__ labels, const floa
         const long long lab = labels[((long long)n * g.H + Y) * g.W + X];
         const bool valid = lab != (long long)g.ignore_index && lab >= 0 && lab < NC;
         float J[NC];
-        joint_head0(g, n, Y, X, hi_cls, M, J);
+        joint_head<kHead>(g, n, Y, X, hi_cls, M, J);
 #pragma unroll
         for (int c = 0; c < NC; ++c) {
           ap[c] += (valid ? sigmoidf_(J[c]) : 0.f) + kClipMin;
-          al[c] += (valid && (int)lab == c) ? 1.f : 0.f;
+          if (kHead == 0) al[c] += (valid && (int)lab == c) ? 1.f : 0.f;
         }
       }
     }
     float* po = pr_pool + idx * LD;
-    float* lo = la_pool + idx * LD;
 #pragma unroll
-    for (int c = 0; c < NC; ++c) { po[c] = ap[c] * 0.0625f; lo[c] = al[c] * 0.0625f; }
+    for (int c = 0; c < NC; ++c) po[c] = ap[c] * 0.0625f;
     po[NC] = 0.f;
-    lo[NC] = 0.f;
+    if (kHead == 0) {
+      float* lo = la_pool + idx * LD;
+#pragma unroll
+      for (int c = 0; c < NC; ++c) lo[c] = al[c] * 0.0625f;
+      lo[NC] = 0.f;
+    }
   }
 }
 
@@ -252,9 +259,20 @@ extern "C" int b200seg_rmi_pool(const b200seg_mscale_desc* d, const int64_t* lab
   if (!d || !labels || !hi_cls || !pr_pool || !la_pool || (d->hm > 0 && !mid)) return B200SEG_E_BADARG;
   if (d->h < 12 || d->w < 12) return B200SEG_E_BADARG;     // at least one 3x3 view of pooled cells
   const int Hp = d->h / 4 + 1, Wp = d->w / 4 + 1;
-  cudaError_t e = launch_k(rmi_pool_kernel, dim3(blocks_for_total((long long)d->n * Hp * Wp, 128)), dim3(128), 0,
+  cudaError_t e = launch_k(rmi_pool_kernel<0>, dim3(blocks_for_total((long long)d->n * Hp * Wp, 128)), dim3(128), 0,
                            (cudaStream_t)stream, to_geom(d), (const long long*)labels, hi_cls, mid, pr_pool, la_pool,
                            Hp, Wp);
+  return e == cudaSuccess ? 0 : (int)e;
+}
+
+extern "C" int b200seg_rmi_pool_aux(const b200seg_mscale_desc* d, const int64_t* labels, const float* hi_aux,
+                                    const float* mid, float* pr_pool, void* stream) {
+  if (!d || !labels || !hi_aux || !pr_pool || d->nheads < 2 || (d->hm > 0 && !mid)) return B200SEG_E_BADARG;
+  if (d->h < 12 || d->w < 12) return B200SEG_E_BADARG;
+  const int Hp = d->h / 4 + 1, Wp = d->w / 4 + 1;
+  cudaError_t e = launch_k(rmi_pool_kernel<1>, dim3(blocks_for_total((long long)d->n * Hp * Wp, 128)), dim3(128), 0,
+                           (cudaStream_t)stream, to_geom(d), (const long long*)labels, hi_aux, mid, pr_pool,
+                           (float*)nullptr, Hp, Wp);
   return e == cudaSuccess ? 0 : (int)e;
 }
 

@@ -30,8 +30,7 @@ def build(arch, num_classes, criterion):
             raise NotImplementedError("align_corners=True is not covered by the B200 resampling kernels")
         if cfg.MODEL.OCR_ASPP or cfg.MODEL.MSCALE_OLDARCH or not cfg.MODEL.MSCALE_INNER_3x3 or cfg.MODEL.MSCALE_DROPOUT:
             raise NotImplementedError("only the default OCR / attention-head configuration is on the hot path")
-        if cfg.LOSS.OCR_AUX_RMI:
-            raise NotImplementedError("OCR_AUX_RMI is not covered")
+        kw["ocr_aux_rmi"] = bool(cfg.LOSS.OCR_AUX_RMI)
         # cfg.MODEL.BNFUNC (config.py:216-225: apex.parallel.SyncBatchNorm under --syncbn --apex, else BatchNorm2d)
         # decides whether BatchNorm statistics span the data-parallel group
         bnfunc = getattr(cfg.MODEL, "BNFUNC", None)
