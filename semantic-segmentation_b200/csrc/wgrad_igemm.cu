@@ -16,6 +16,15 @@
 //   * splits  > 1 (high-resolution narrow layers): units store fp32 slabs and wgrad_reduce_kernel sums the splits in a
 //     fixed order (deterministic) with coalesced float4 traffic.
 // The decomposition (N tile width, taps per group, splits) is picked per layer by a small cost model (wgrad_plan).
+//
+// MMA issue: the kernel is instantiated per W16 = min(Cin, ntile_w) / 16 (1 .. 16) and its tap loop is unrolled up to
+// the most taps a unit can hold (min(9, 16 / W16)), so every MMA's width (W16 / 4 n64 MMAs and at most one n16/n32/n48
+// tail) and accumulator offset (tap * W16 * 16 columns) are compile-time constants. Only the unit's tap count (a short
+// last tap group) is tested at run time, between the (pixel tile, tap) MMA groups; nothing branches between an MMA and
+// the commit of its group. So ptxas keeps the accumulators in registers without spills and keeps one group in flight
+// under the next (wgmma_wait<1>); tests/test_wgrad_sass.py checks the compiled code for both. The last N tile of a
+// multi-tile layer (720 channels: 256, 256, 208) runs the full W16 width and drops the extra columns in the epilogue
+// (2.6% more MMA work over the weight gradients of the two-scale 1024x2048 step).
 // The step folds the OHWI accumulators into the OIHW master gradients once, at the end (grad_fold_kernel).
 // Replaces cuDNN convolution_backward (weight part) behind every nn.Conv2d listed in SURVEY.md §2b K1-K5.
 #include "ptx.cuh"
@@ -24,6 +33,7 @@
 #include "conv_common.h"
 #include "conv_epi.cuh"
 #include "../../include/b200seg.h"
+#include <utility>
 
 namespace b200seg {
 
@@ -45,7 +55,8 @@ constexpr int kABlock = 128 * 128;   // 128 pixel rows x 64 channels bf16
 constexpr int kMaxBSlots = 6;
 constexpr int kWAccCols = 256;       // accumulator columns per consumer thread row (128 registers)
 
-// one MN-major MMA of width 16 * w (w <= 4 blocks: inside one 64-channel swizzle atom)
+// one MN-major MMA of width 16 * w (w <= 4 blocks: inside one 64-channel swizzle atom). Every call site passes a
+// compile-time w (fully unrolled loops), so the selection folds away.
 __device__ __forceinline__ void wgmma_mn(float* d, int w, uint64_t a, uint64_t b, uint32_t scale_d) {
   if (w >= 4) wgmma_n64<1, 1>(d, a, b, scale_d);
   else if (w == 3) wgmma_n48<1, 1>(d, a, b, scale_d);
@@ -53,10 +64,13 @@ __device__ __forceinline__ void wgmma_mn(float* d, int w, uint64_t a, uint64_t b
   else wgmma_n16<1, 1>(d, a, b, scale_d);
 }
 
+// W16 = Nmax / 16: 16-column blocks of one tap's accumulator (Nmax = min(Cin, ntile_w), the unit slab's row pitch).
+// p is a __grid_constant__ so the lambdas can capture it by reference without a stack copy.
+template <int W16>
 __global__ void __launch_bounds__(kWThreads, 1)
 wgrad_igemm_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constant__ CUtensorMap tmX,
-                   const WgradParams p, float* __restrict__ ws, float* __restrict__ dw) {
-  constexpr int NB = kWAccCols / 16;
+                   const __grid_constant__ WgradParams p, float* __restrict__ ws, float* __restrict__ dw) {
+  constexpr int kMaxTaps = kWAccCols / 16 / W16 < 9 ? kWAccCols / 16 / W16 : 9;   // taps of one unit (ksize <= 3)
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* a_base = smem;                               // 2 slots
@@ -131,75 +145,78 @@ wgrad_igemm_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_consta
     // 16 pixels per K step = 2048 B of both operands; 8-pixel groups 1024 B apart; 64-channel atoms kABlock apart
     const uint64_t tmpl = make_smem_desc(0, kABlock, 1024, 1);
     const uint32_t a0 = smem_u32(a_base) + g * kABlock, b0 = smem_u32(b_base);
-    float acc[NB * 8];
+    // thread rows: output channels co0 (+8); block (tap tl, 16 columns c): columns 16c + 8h + 2(lane % 4) + {0, 1}
+    const int row0 = (int)(g * 64 + (warp & 3) * 16 + (lane >> 2));
     int a_slot = 0, b_slot = 0;
     uint32_t a_phase = 0, b_phase = 0;
     for (int unit = blockIdx.x; unit < p.total_units; unit += gridDim.x) {
       int m_tile, n_tile, tg, split;
       decode(unit, m_tile, n_tile, tg, split);
       const int n0 = n_tile * p.ntile_w;
-      const int Nn = min(p.ntile_w, p.Cin - n0);         // multiple of 16
-      const int nb16 = Nn >> 4;
-      const int tap0 = tg * p.taps_per_group, tap1 = min(p.taps, tap0 + p.taps_per_group);
+      const int Nn = min(p.ntile_w, p.Cin - n0);         // multiple of 16; < 16 * W16 only in the last N tile
+      const int tap0 = tg * p.taps_per_group, ntaps = min(p.taps, tap0 + p.taps_per_group) - tap0;
       const bool active = g == 0 || (p.Cout - m_tile * 128) > 64;   // this warpgroup's dy block holds real channels
-      PendingRelease pend;
+      // Each MMA spans all W16 blocks even in a narrower last N tile: an output column depends on its own B column
+      // only, so the columns >= Nn (stale or zero-filled shared memory) are computed and dropped by the epilogue.
+      float acc[kMaxTaps * W16 * 8];
+      uint32_t pend_b = 0, pend_a = 0;   // empty barriers of the group still in flight (shared addresses, 0: none)
       uint32_t started = 0;
       for (int t = split; t < p.pix_tiles; t += p.splits) {
         mbar_wait(&a_full[a_slot], a_phase);
         const uint64_t ad = tmpl + (uint64_t)((a0 + (uint32_t)a_slot * (uint32_t)p.a_slot_bytes) >> 4);
-        for (int tap = tap0; tap < tap1; ++tap) {
-          const int tl = tap - tap0;
+#pragma unroll
+        for (int tl = 0; tl < kMaxTaps; ++tl) {
+          if (tl >= ntaps) break;
           mbar_wait(&b_full[b_slot], b_phase);
           const uint64_t bd = tmpl + (uint64_t)((b0 + (uint32_t)b_slot * (uint32_t)p.b_slot_bytes) >> 4);
           if (active) {
             wgmma_fence();
+#pragma unroll
             for (int k = 0; k < 8; ++k) {
 #pragma unroll
-              for (int j = 0; j < NB; ++j) {
-                const int c = j - tl * nb16;
-                if (c >= 0 && c < nb16 && (c & 3) == 0)
-                  wgmma_mn(&acc[8 * j], nb16 - c, ad + (uint64_t)(k * 128),
-                           bd + (uint64_t)(k * 128 + (c >> 2) * (kABlock >> 4)), started | (uint32_t)k);
-              }
+              for (int c = 0; c < W16; c += 4)
+                wgmma_mn(&acc[8 * (tl * W16 + c)], W16 - c, ad + (uint64_t)(k * 128),
+                         bd + (uint64_t)(k * 128 + (c >> 2) * (kABlock >> 4)), started | (uint32_t)k);
             }
             wgmma_commit();
             wgmma_wait<1>();
           }
-          pend.release(leader);
-          pend.bar0 = &b_empty[b_slot];
-          if (tap == tap1 - 1) pend.bar1 = &a_empty[a_slot];
+          if (leader && pend_b) mbar_arrive_at(pend_b);
+          if (leader && pend_a) mbar_arrive_at(pend_a);
+          pend_b = smem_u32(&b_empty[b_slot]);
+          pend_a = tl == ntaps - 1 ? smem_u32(&a_empty[a_slot]) : 0u;
           if (++b_slot == p.b_slots) { b_slot = 0; b_phase ^= 1; }
         }
         if (++a_slot == 2) { a_slot = 0; a_phase ^= 1; }
         started = 1;
       }
       wgmma_wait<0>();
-      pend.release(leader);
+      if (leader && pend_b) mbar_arrive_at(pend_b);
+      if (leader && pend_a) mbar_arrive_at(pend_a);
       if (!started || !active) continue;
-      // thread rows: output channels co0 (+8); block j = (tap tl, 16 columns c): columns 16c + 8h + 2(lane % 4) + {0, 1}
-      const int row0 = (int)(g * 64 + (warp & 3) * 16 + (lane >> 2));
 #pragma unroll
-      for (int j = 0; j < NB; ++j) {
-        if (j >= (tap1 - tap0) * nb16) break;
-        const int tl = j / nb16, c = j - tl * nb16;
+      for (int tl = 0; tl < kMaxTaps; ++tl) {
+        if (tl >= ntaps) break;
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int col = c * 16 + 8 * h + 2 * (int)(lane & 3);
+        for (int c = 0; c < W16; ++c) {
+          if (c * 16 >= Nn) break;
 #pragma unroll
-          for (int r = 0; r < 2; ++r) {
-            const int row = row0 + 8 * r, co = m_tile * 128 + row;
-            if (co >= p.Cout) continue;
-            const float v0 = acc[8 * j + 4 * h + 2 * r], v1 = acc[8 * j + 4 * h + 2 * r + 1];
-            if (p.direct) {
-              // the only unit that touches these gradient elements: fire-and-forget reductions
-              float* dst = dw + ((size_t)co * p.taps + tap0 + tl) * p.Cin + n0 + col;
-              atomicAdd(dst, v0);
-              atomicAdd(dst + 1, v1);
-            } else {
-              // per-unit slab [tap_local][128 rows][unit_n] fp32, summed by wgrad_reduce_kernel
-              float2* dst = reinterpret_cast<float2*>(ws + (size_t)unit * p.unit_stride +
-                                                      ((size_t)tl * 128 + row) * p.unit_n + col);
-              *dst = make_float2(v0, v1);
+          for (int h = 0; h < 2; ++h) {
+            const int col = c * 16 + 8 * h + 2 * (int)(lane & 3);
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+              const int row = row0 + 8 * r, co = m_tile * 128 + row;
+              if (co >= p.Cout) continue;
+              const float v0 = acc[8 * (tl * W16 + c) + 4 * h + 2 * r], v1 = acc[8 * (tl * W16 + c) + 4 * h + 2 * r + 1];
+              if (p.direct) {
+                // the only unit that touches these gradient elements: a fire-and-forget reduction
+                red_add_v2(dw + ((size_t)co * p.taps + tap0 + tl) * p.Cin + n0 + col, v0, v1);
+              } else {
+                // per-unit slab [tap_local][128 rows][unit_n] fp32, summed by wgrad_reduce_kernel
+                float2* dst = reinterpret_cast<float2*>(ws + (size_t)unit * p.unit_stride +
+                                                        ((size_t)tl * 128 + row) * p.unit_n + col);
+                *dst = make_float2(v0, v1);
+              }
             }
           }
         }
@@ -208,7 +225,6 @@ wgrad_igemm_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_consta
     if (g == 0 && leader) pdl_launch_late();
   }
 }
-
 
 // dw[co][tap][ci] += sum over the pixel splits of the unit slabs, splits summed in a fixed order (deterministic).
 // One thread block = 32 consecutive float4 of an item's [tap_local][row][col] index space (coalesced 512-byte slab reads)
@@ -342,6 +358,13 @@ publish_grads_kernel(float* __restrict__ dst, const float* __restrict__ src, lon
 }  // namespace b200seg
 
 using namespace b200seg;
+
+using WgradKernel = void (*)(CUtensorMap, CUtensorMap, WgradParams, float*, float*);
+template <int... I>
+static WgradKernel wgrad_kernel(int w16, std::integer_sequence<int, I...>) {
+  static constexpr WgradKernel k[] = {wgrad_igemm_kernel<I + 1>...};
+  return k[w16 - 1];
+}
 
 static int wgrad_grid(const WgradParams& p) { return p.total_units < B200SEG_MAX_CTAS ? p.total_units : B200SEG_MAX_CTAS; }
 
@@ -485,16 +508,18 @@ extern "C" int b200seg_conv2d_wgrad(const b200seg_conv_desc* d, const void* x, c
     int rc = encode_bf16(&tmX, x, 4, dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(wgrad_igemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  const int w16 = p.unit_n / 16;                  // 1 .. 16 (the planner caps the N tile at kWAccCols columns)
+  const WgradKernel kernel = wgrad_kernel(w16, std::make_integer_sequence<int, kWAccCols / 16>());
+  static bool attr_set[kWAccCols / 16] = {};
+  if (!attr_set[w16 - 1]) {
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) return (int)e;
-    e = cudaFuncSetAttribute(wgrad_igemm_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     if (e != cudaSuccess) return (int)e;
-    attr_set = true;
+    attr_set[w16 - 1] = true;
   }
-  cudaError_t e = launch_k(wgrad_igemm_kernel, dim3(wgrad_grid(p)), dim3(kWThreads), smem_bytes, (cudaStream_t)stream, tmDy,
-                           tmX, p, (float*)workspace, dw_ohwi);
+  cudaError_t e = launch_k(kernel, dim3(wgrad_grid(p)), dim3(kWThreads), smem_bytes, (cudaStream_t)stream, tmDy, tmX, p,
+                           (float*)workspace, dw_ohwi);
   if (e != cudaSuccess) return (int)e;
   if (p.direct) return 0;
   const int items = p.m_tiles * p.n_tiles * p.tap_groups;
