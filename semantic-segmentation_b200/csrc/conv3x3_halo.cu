@@ -13,6 +13,11 @@
 // Weights: resident in shared memory for the whole persistent CTA when they fit (C <= 96: the HBM-bound layers), else
 // streamed per (chunk, tap) through an mbarrier ring. The Cout tile (BN) is chosen per launch by a small cost model so
 // that low-resolution layers still spread over the SMs (a 16x32x384 layer has 4 pixel tiles but 6 x 64-wide Cout tiles).
+// MMA issue: the kernel is instantiated per (OCC, NB16 = BN / 16), so every MMA's width (NB16 / 4 n64 MMAs and at most one
+// n16/n32/n48 tail) and accumulator offset are compile-time constants. A chunk's K steps (4, or 1-3 in the last chunk of
+// a Cin that is not a multiple of 64) select one of four fully unrolled group bodies before the fence, so nothing
+// between a fence and its commit depends on a run-time value and one group stays in flight under the next
+// (wgmma_wait<1>); tests/test_conv_sass.py checks the compiled code.
 // Replaces cuDNN fwd/dgrad behind the 3x3 stride-1 convolutions of network/hrnetv2.py:31-34 (BasicBlock), :76
 // (Bottleneck), network/ocrnet.py:54-57 (conv3x3_ocr) and network/utils.py:348-356 (attention head).
 #include <cstdio>
@@ -24,6 +29,8 @@
 #include "launch.h"
 #include "../../include/b200seg.h"
 #include <cstdlib>
+#include <type_traits>
+#include <utility>
 
 namespace b200seg {
 
@@ -33,7 +40,7 @@ struct HaloParams {
   int ksteps_last;             // K=16 steps in the last chunk
   int BN, n_tiles, cout_pad;   // cout_pad = roundup16(Cout): row pitch of the statistics partials
   int tiles_h, tiles_w, total_tiles;
-  int y_ld, has_bias, emit_stats, addend_ld;
+  int y_ld, emit_stats, addend_ld;
   int resident;                // weights stay in smem for the CTA lifetime
   int a_slots, b_slots;        // ring depths (b_slots unused when resident)
   int b_tile_bytes;            // BN * 128 rounded to 1024
@@ -46,13 +53,14 @@ constexpr int kPlaneBytes = kHaloH * kHaloW * 16;   // one 8-channel plane of th
 constexpr int kPlane = 2944;                         // plane pitch: TMA destinations are 128-byte aligned
 constexpr int kMaxASlots = 4, kMaxBSlots2 = 8;
 
-// OCC: CTAs per SM; the two-per-SM build holds at most 128 accumulator columns (64 registers per consumer thread).
-template <int OCC>
+// OCC: CTAs per SM; NB16 = BN / 16: 16-column accumulator blocks of the Cout tile (the two-per-SM build exists for
+// NB16 <= 8: at most 128 accumulator columns, 64 registers per consumer thread).
+template <int OCC, int NB16>
 __global__ void __launch_bounds__(kHThreads, OCC)
 conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                    const HaloParams p, __nv_bfloat16* __restrict__ y, const float* __restrict__ bias,
+                    const __grid_constant__ HaloParams p, __nv_bfloat16* __restrict__ y, const float* __restrict__ bias,
                     float* __restrict__ stats_partials, const __nv_bfloat16* __restrict__ addend, const BnFoldDev fold) {
-  constexpr int NB = OCC == 2 ? 8 : 16;    // 16-column accumulator blocks
+  static_assert(NB16 >= 1 && NB16 <= (OCC == 2 ? 8 : 16), "accumulator columns exceed the register budget");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* a_base = smem;
@@ -127,57 +135,79 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     // ------------------------------------------------------------------ consumers: MMA + epilogue
     const uint32_t g = warp >> 2;               // warpgroup: tile rows 8g .. 8g + 7
     const bool leader = (threadIdx.x & 127) == 0;
-    float* my_stats = s_stats + (size_t)warp * 2 * p.cout_pad;
+    // barriers by shared-memory address: a_full[s] = bar0 + 8 s, a_empty = + 8 kMaxASlots, b_full / b_empty after them
+    const uint32_t bar0 = smem_u32(bars);
+    const uint32_t a_empty0 = bar0 + 8 * kMaxASlots, b_full0 = bar0 + 16 * kMaxASlots, b_empty0 = b_full0 + 8 * kMaxBSlots2;
     const uint64_t a_tmpl = make_smem_desc(0, kPlane, kHaloW * 16, 0);
     const uint64_t b_tmpl = make_smem_desc(0, p.BN * 16, 128, 0);
     const uint32_t a0 = smem_u32(a_base) + g * 8 * kHaloW * 16, b0 = smem_u32(b_base);
     const uint32_t b64 = (64 * 16) >> 4;                  // 64 weight rows of 16 bytes
     const uint32_t bk16 = (uint32_t)(2 * p.BN * 16) >> 4;  // next K = 16 step: two channel-group planes
     const uint32_t ak16 = (2 * kPlane) >> 4;
-    const int nb16 = p.BN >> 4;
     const int last = p.cchunks - 1;
-    ConvEpi e{y, p.has_bias ? bias : nullptr, addend, p.y_ld, p.addend_ld, 0, p.Cout, p.emit_stats, p.cout_pad};
-    float acc[NB * 8];
-    int a_slot = 0, b_slot = 0;
-    uint32_t a_phase = 0, b_phase = 0;
-    if (p.resident) mbar_wait(&b_full[0], 0);
+    // ring positions: slot in bits 0-7, phase in bit 8 (one register per ring next to the accumulators)
+    uint32_t a_pos = 0, b_pos = 0;
+    auto advance = [](uint32_t pos, int slots) { return (int)(pos & 0xff) + 1 == slots ? (pos & 0x100) ^ 0x100 : pos + 1; };
+    if (p.resident) mbar_wait_at(b_full0, 0);
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      // Defined afresh per tile: the wgmma operands read the accumulators, so without this every accumulator of the
+      // previous tile would stay live through its whole epilogue (the first MMA of a tile uses scale-d 0 and ignores
+      // these zeros).
+      float acc[NB16 * 8];
+#pragma unroll
+      for (int i = 0; i < NB16 * 8; ++i) acc[i] = 0.f;
       PendingRelease pend;
       for (int cc = 0; cc <= last; ++cc) {
-        mbar_wait(&a_full[a_slot], a_phase);
-        const uint64_t ad = a_tmpl + (uint64_t)((a0 + (uint32_t)a_slot * kASlotBytes) >> 4);
-        const int ks = (cc == last) ? p.ksteps_last : 4;
-        if (p.resident) {
-          wgmma_fence();
-          for (int t = 0; t < 9; ++t) {
-            const int kh = t / 3, kw = t - kh * 3;
-            const uint64_t at = ad + (uint64_t)(kh * kHaloW + kw);     // (kh*10 + kw) pixels of 16 B
-            const uint64_t bt = b_tmpl + (uint64_t)((b0 + (uint32_t)(cc * 9 + t) * (uint32_t)p.b_tile_bytes) >> 4);
-            for (int k = 0; k < ks; ++k)
-              wgmma_row<NB, 0, 0>(acc, nb16, at + (uint64_t)(k * ak16), bt + (uint64_t)(k * bk16), b64, (cc | t | k) != 0);
-          }
-          wgmma_commit();
-          wgmma_wait<1>();
-          pend.release(leader);
-          pend.bar0 = &a_empty[a_slot];
-        } else {
-          for (int t = 0; t < 9; ++t) {
-            const int kh = t / 3, kw = t - kh * 3;
-            mbar_wait(&b_full[b_slot], b_phase);
-            const uint64_t at = ad + (uint64_t)(kh * kHaloW + kw);
-            const uint64_t bt = b_tmpl + (uint64_t)((b0 + (uint32_t)b_slot * (uint32_t)p.b_tile_bytes) >> 4);
+        const uint32_t a_slot = a_pos & 0xff;
+        mbar_wait_at(bar0 + 8 * a_slot, a_pos >> 8);
+        const uint64_t ad = a_tmpl + (uint64_t)((a0 + a_slot * kASlotBytes) >> 4);
+        // The MMAs of one chunk with KS = 16-channel K steps, fully unrolled: nothing between a fence and its commit
+        // depends on a run-time value, so ptxas keeps the accumulators in registers and the group in flight.
+        auto chunk = [&](auto ks_const) {
+          constexpr int KS = decltype(ks_const)::value;
+          if (p.resident) {
             wgmma_fence();
-            for (int k = 0; k < ks; ++k)
-              wgmma_row<NB, 0, 0>(acc, nb16, at + (uint64_t)(k * ak16), bt + (uint64_t)(k * bk16), b64, (cc | t | k) != 0);
+#pragma unroll
+            for (int t = 0; t < 9; ++t) {
+              const int kh = t / 3, kw = t - kh * 3;
+              const uint64_t at = ad + (uint64_t)(kh * kHaloW + kw);     // (kh*10 + kw) pixels of 16 B
+              const uint64_t bt = b_tmpl + (uint64_t)((b0 + (uint32_t)(cc * 9 + t) * (uint32_t)p.b_tile_bytes) >> 4);
+#pragma unroll
+              for (int k = 0; k < KS; ++k)
+                wgmma_row<NB16, 0, 0>(acc, at + (uint64_t)(k * ak16), bt + (uint64_t)(k * bk16), b64, (cc | t | k) != 0);
+            }
             wgmma_commit();
             wgmma_wait<1>();
             pend.release(leader);
-            pend.bar0 = &b_empty[b_slot];
-            if (t == 8) pend.bar1 = &a_empty[a_slot];
-            if (++b_slot == p.b_slots) { b_slot = 0; b_phase ^= 1; }
+            pend.bar0 = a_empty0 + 8 * a_slot;
+          } else {
+            for (int t = 0; t < 9; ++t) {
+              const int kh = t / 3, kw = t - kh * 3;
+              const uint32_t b_slot = b_pos & 0xff;
+              mbar_wait_at(b_full0 + 8 * b_slot, b_pos >> 8);
+              const uint64_t at = ad + (uint64_t)(kh * kHaloW + kw);
+              const uint64_t bt = b_tmpl + (uint64_t)((b0 + b_slot * (uint32_t)p.b_tile_bytes) >> 4);
+              wgmma_fence();
+#pragma unroll
+              for (int k = 0; k < KS; ++k)
+                wgmma_row<NB16, 0, 0>(acc, at + (uint64_t)(k * ak16), bt + (uint64_t)(k * bk16), b64, (cc | t | k) != 0);
+              wgmma_commit();
+              wgmma_wait<1>();
+              pend.release(leader);
+              pend.bar0 = b_empty0 + 8 * b_slot;
+              if (t == 8) pend.bar1 = a_empty0 + 8 * a_slot;
+              b_pos = advance(b_pos, p.b_slots);
+            }
           }
+        };
+        // every chunk has 4 K steps except the last one of a Cin that is not a multiple of 64 (48: 3, 96: 2, 720: 1)
+        switch (cc == last ? p.ksteps_last : 4) {
+          case 1: chunk(std::integral_constant<int, 1>()); break;
+          case 2: chunk(std::integral_constant<int, 2>()); break;
+          case 3: chunk(std::integral_constant<int, 3>()); break;
+          default: chunk(std::integral_constant<int, 4>()); break;
         }
-        if (++a_slot == p.a_slots) { a_slot = 0; a_phase ^= 1; }
+        a_pos = advance(a_pos, p.a_slots);
       }
       wgmma_wait<0>();
       pend.release(leader);
@@ -197,7 +227,8 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         valid[r] = (ho < p.H) && (wo < p.W);
         pix[r] = ((size_t)img * p.H + ho) * p.W + wo;
       }
-      conv_epilogue<NB>(acc, nb16, n_tile * p.BN, valid, pix, e, fold, my_stats, lane);
+      const ConvEpi e{y, bias, addend, p.y_ld, p.addend_ld, 0, p.Cout, p.emit_stats, p.cout_pad};
+      conv_epilogue<NB16>(acc, n_tile * p.BN, valid, pix, e, fold, smem_u32(s_stats) + warp * 8 * p.cout_pad, lane);
     }
   }
 
@@ -318,6 +349,27 @@ int conv3x3_halo_plan_info(int n, int h, int w, int cin, int cout, int32_t* out)
   return 0;
 }
 
+// The instantiation of a launch: CTAs per SM (occ) and Cout tile width (nb16 = BN / 16).
+using HaloKernel = void (*)(CUtensorMap, CUtensorMap, HaloParams, __nv_bfloat16*, const float*, float*,
+                            const __nv_bfloat16*, BnFoldDev);
+template <int OCC, int... I>
+static HaloKernel halo_kernel_of(int nb16, std::integer_sequence<int, I...>) {
+  static constexpr HaloKernel k[] = {conv3x3_halo_kernel<OCC, I + 1>...};
+  return k[nb16 - 1];
+}
+static HaloKernel halo_kernel(int occ, int nb16) {
+  return occ == 2 ? halo_kernel_of<2>(nb16, std::make_integer_sequence<int, 8>())
+                  : halo_kernel_of<1>(nb16, std::make_integer_sequence<int, 16>());
+}
+static cudaError_t halo_set_attributes(HaloKernel k, int occ) {
+  cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       occ == 2 ? (int)kHalfSmBudget : 227 * 1024);
+  // two CTAs per SM need (almost) the whole 228 KB as shared memory: ask for the maximum carve-out explicitly
+  if (e == cudaSuccess && occ == 2)
+    e = cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  return e;
+}
+
 int make_bn_fold(const b200seg_bn_fold* f, int cout, BnFoldDev* out);
 int conv3x3_halo_launch(int n, int h, int w, int cin, int in_ld, const void* in, int cout, const void* wts,
                         const float* bias, void* out, int out_ld, float* stats_partials, int32_t* stats_grid,
@@ -335,7 +387,7 @@ int conv3x3_halo_launch(int n, int h, int w, int cin, int in_ld, const void* in,
   size_t smem_bytes;
   int grid, occ;
   if (int rc = halo_plan(n, h, w, cin, cout, p, smem_bytes, grid, occ)) return rc;
-  p.y_ld = out_ld; p.has_bias = bias != nullptr; p.emit_stats = emit_stats; p.addend_ld = addend_ld;
+  p.y_ld = out_ld; p.emit_stats = emit_stats; p.addend_ld = addend_ld;
   if (stats_grid) *stats_grid = grid;
   if (!in || !wts || !out) return B200SEG_E_BADARG;
   if ((reinterpret_cast<uintptr_t>(in) & 15) || (reinterpret_cast<uintptr_t>(wts) & 15) ||
@@ -356,37 +408,28 @@ int conv3x3_halo_launch(int n, int h, int w, int cin, int in_ld, const void* in,
     int rc = encode_bf16(&tmB, wts, 3, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_NONE);
     if (rc) return rc;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv3x3_halo_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  const HaloKernel kernel = halo_kernel(occ, p.BN / 16);
+  static bool attr_set[2][16] = {};
+  if (!attr_set[occ - 1][p.BN / 16 - 1]) {
+    cudaError_t e = halo_set_attributes(kernel, occ);
     if (e != cudaSuccess) return (int)e;
-    e = cudaFuncSetAttribute(conv3x3_halo_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHalfSmBudget);
-    if (e != cudaSuccess) return (int)e;
-    // two CTAs per SM need (almost) the whole 228 KB as shared memory: ask for the maximum carve-out explicitly
-    e = cudaFuncSetAttribute(conv3x3_halo_kernel<2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    if (e != cudaSuccess) return (int)e;
-    attr_set = true;
+    attr_set[occ - 1][p.BN / 16 - 1] = true;
   }
-  cudaError_t e =
-      occ == 2 ? launch_k(conv3x3_halo_kernel<2>, dim3(grid), dim3(kHThreads), smem_bytes, stream, tmA, tmB, p,
-                          (__nv_bfloat16*)out, bias, stats_partials, (const __nv_bfloat16*)addend, fd)
-               : launch_k(conv3x3_halo_kernel<1>, dim3(grid), dim3(kHThreads), smem_bytes, stream, tmA, tmB, p,
-                          (__nv_bfloat16*)out, bias, stats_partials, (const __nv_bfloat16*)addend, fd);
+  cudaError_t e = launch_k(kernel, dim3(grid), dim3(kHThreads), smem_bytes, stream, tmA, tmB, p, (__nv_bfloat16*)out,
+                           bias, stats_partials, (const __nv_bfloat16*)addend, fd);
   return e == cudaSuccess ? 0 : (int)e;
 }
 
 
 // Diagnostics: CTAs per SM the runtime grants the co-resident (OCC = 2) and the full-SM (OCC = 1) build of the two
-// convolution kernels for a given dynamic shared-memory size (registers, shared-memory carve-out, barriers all included).
+// convolution kernels for a given dynamic shared-memory size (registers, shared-memory carve-out, barriers all included),
+// at the widest Cout tile of each build (NB16 = 8 / 16: the most accumulator registers).
 int conv_igemm_occupancy(int occ_variant, int smem_bytes);
 int conv3x3_halo_occupancy(int occ_variant, int smem_bytes) {
   int nb = -1;
-  cudaFuncSetAttribute(conv3x3_halo_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(conv3x3_halo_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHalfSmBudget);
-  cudaFuncSetAttribute(conv3x3_halo_kernel<2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  cudaError_t e = occ_variant == 2
-      ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, conv3x3_halo_kernel<2>, kHThreads, (size_t)smem_bytes)
-      : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, conv3x3_halo_kernel<1>, kHThreads, (size_t)smem_bytes);
+  const HaloKernel k = halo_kernel(occ_variant, occ_variant == 2 ? 8 : 16);
+  halo_set_attributes(k, occ_variant);
+  cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k, kHThreads, (size_t)smem_bytes);
   return e == cudaSuccess ? nb : -(int)e;
 }
 
@@ -417,9 +460,14 @@ extern "C" void b200seg_debug_occupancy_report(void) {
          "max blocks/SM %d max threads/SM %d\n", pr.name, pr.multiProcessorCount, pr.regsPerMultiprocessor,
          pr.regsPerBlock, pr.sharedMemPerMultiprocessor, pr.sharedMemPerBlockOptin, pr.reservedSharedMemPerBlock,
          pr.maxBlocksPerMultiProcessor, pr.maxThreadsPerMultiProcessor);
-  b200seg::conv3x3_halo_occupancy(2, 1024);     // sets the attributes of both builds
-  b200seg::occupancy_report_one("conv3x3_halo_kernel<2>", b200seg::conv3x3_halo_kernel<2>, b200seg::kHThreads);
-  b200seg::occupancy_report_one("conv3x3_halo_kernel<1>", b200seg::conv3x3_halo_kernel<1>, b200seg::kHThreads);
+  for (int occ = 2; occ >= 1; --occ)
+    for (int nb16 = 1; nb16 <= (occ == 2 ? 8 : 16); ++nb16) {
+      char name[64];
+      snprintf(name, sizeof(name), "conv3x3_halo_kernel<%d, %d>", occ, nb16);
+      const b200seg::HaloKernel k = b200seg::halo_kernel(occ, nb16);
+      b200seg::halo_set_attributes(k, occ);
+      b200seg::occupancy_report_one(name, k, b200seg::kHThreads);
+    }
   b200seg::conv_igemm_occupancy_report();
   fflush(stdout);
 }

@@ -1,5 +1,5 @@
 // Shared pieces of the two forward / data-gradient convolution kernels (conv_igemm.cu, conv3x3_halo.cu):
-//   * the MMA of one K = 16 step over all N columns of a warpgroup tile (64 rows x 16 * nb16 columns), and
+//   * the MMA of one K = 16 step over all N columns of a warpgroup tile (64 rows x 16 * NB16 columns), and
 //   * the epilogue of a warpgroup tile straight from the wgmma accumulator fragment (ptx.cuh).
 #pragma once
 #include <cuda_bf16.h>
@@ -8,18 +8,18 @@
 
 namespace b200seg {
 
-// Columns [0, 16 * nb16) of acc (NB = 16-column blocks the kernel build holds): one MMA per 64-column group, narrower for
-// the tail. b64 = descriptor distance between 64-column groups of the B operand (16-byte units).
-template <int NB, int TA, int TB>
-__device__ __forceinline__ void wgmma_row(float (&acc)[NB * 8], int nb16, uint64_t a, uint64_t b, uint32_t b64,
-                                          uint32_t scale_d) {
+// Columns [0, 16 * NB16) of acc: NB16 / 4 n64 MMAs and at most one n16/n32/n48 tail, all at compile-time accumulator
+// offsets (the loop unrolls, so the width selection folds away). b64 = descriptor distance between 64-column groups of the
+// B operand (16-byte units).
+template <int NB16, int TA, int TB>
+__device__ __forceinline__ void wgmma_row(float (&acc)[NB16 * 8], uint64_t a, uint64_t b, uint32_t b64, uint32_t scale_d) {
 #pragma unroll
-  for (int j = 0; j < NB; j += 4) {
+  for (int j = 0; j < NB16; j += 4) {
     const uint64_t bj = b + (uint64_t)((j / 4) * b64);
-    if (j + 4 <= nb16) wgmma_n64<TA, TB>(&acc[8 * j], a, bj, scale_d);
-    else if (j + 3 == nb16) wgmma_n48<TA, TB>(&acc[8 * j], a, bj, scale_d);
-    else if (j + 2 == nb16) wgmma_n32<TA, TB>(&acc[8 * j], a, bj, scale_d);
-    else if (j + 1 == nb16) wgmma_n16<TA, TB>(&acc[8 * j], a, bj, scale_d);
+    if (j + 4 <= NB16) wgmma_n64<TA, TB>(&acc[8 * j], a, bj, scale_d);
+    else if (j + 3 == NB16) wgmma_n48<TA, TB>(&acc[8 * j], a, bj, scale_d);
+    else if (j + 2 == NB16) wgmma_n32<TA, TB>(&acc[8 * j], a, bj, scale_d);
+    else wgmma_n16<TA, TB>(&acc[8 * j], a, bj, scale_d);
   }
 }
 
@@ -33,21 +33,23 @@ __device__ __forceinline__ float col_reduce(float v) {
 
 struct ConvEpi {
   void* y;
-  const float* bias;                  // nullable
+  const float* bias;                  // nullable (the host passes null when the layer has no bias)
   const __nv_bfloat16* addend;        // nullable
   int y_ld, addend_ld, out_fp32, Cout, emit_stats, cout_pad;
 };
 
-// Epilogue of a warpgroup tile (columns n0 + [0, 16 * nb16); the thread's two rows at pix[r]): bias, BN affine, addend,
-// ReLU, store; sums / sums of squares of the STORED values into this warp's my_stats[2][cout_pad].
-template <int NB>
-__device__ __forceinline__ void conv_epilogue(const float (&acc)[NB * 8], int nb16, int n0, const bool (&valid)[2],
+// Epilogue of a warpgroup tile (columns n0 + [0, 16 * NB16); the thread's two rows at pix[r]): bias, BN affine, addend,
+// ReLU, store; sums / sums of squares of the STORED values into this warp's statistics [2][cout_pad] fp32 at the shared
+// address my_stats. Columns >= Cout (the last N tile of a layer whose Cout is not a multiple of the tile) are computed by
+// the MMAs and dropped here. The statistics address is 32-bit to keep the state held next to the accumulators small.
+template <int NB16>
+__device__ __forceinline__ void conv_epilogue(const float (&acc)[NB16 * 8], int n0, const bool (&valid)[2],
                                               const size_t (&pix)[2], const ConvEpi& e, const BnFoldDev& fold,
-                                              float* my_stats, uint32_t lane) {
+                                              uint32_t my_stats, uint32_t lane) {
   const bool affine = fold.accum == nullptr && fold.scale != nullptr;   // evaluation: BN folded into the epilogue
 #pragma unroll
-  for (int c = 0; c < 2 * NB; ++c) {
-    if (c >= 2 * nb16 || n0 + 8 * c >= e.Cout) break;     // warp-uniform
+  for (int c = 0; c < 2 * NB16; ++c) {
+    if (n0 + 8 * c >= e.Cout) break;     // warp-uniform
     const int col = n0 + 8 * c + 2 * (int)(lane & 3);
     const bool cv[2] = {col < e.Cout, col + 1 < e.Cout};
     float bi[2] = {0.f, 0.f}, sc[2] = {1.f, 1.f}, sh[2] = {0.f, 0.f};
@@ -87,25 +89,27 @@ __device__ __forceinline__ void conv_epilogue(const float (&acc)[NB * 8], int nb
 #pragma unroll
       for (int q = 0; q < 2; ++q) { s1[q] = col_reduce(s1[q]); s2[q] = col_reduce(s2[q]); }
       if (lane < 4) {
-        my_stats[col] += s1[0];
-        my_stats[col + 1] += s1[1];
-        my_stats[e.cout_pad + col] += s2[0];
-        my_stats[e.cout_pad + col + 1] += s2[1];
+        const uint32_t a1 = my_stats + 4u * (uint32_t)col, a2 = a1 + 4u * (uint32_t)e.cout_pad;
+        st_shared_f32(a1, ld_shared_f32(a1) + s1[0]);
+        st_shared_f32(a1 + 4, ld_shared_f32(a1 + 4) + s1[1]);
+        st_shared_f32(a2, ld_shared_f32(a2) + s2[0]);
+        st_shared_f32(a2 + 4, ld_shared_f32(a2 + 4) + s2[1]);
       }
     }
   }
 }
 
-// Slots of the previous MMA group, freed once it has completed (wgmma_wait<1> after the next commit).
+// Slots of the previous MMA group, freed once it has completed (wgmma_wait<1> after the next commit). The barriers are
+// kept as 32-bit shared-memory addresses (0: none), which holds fewer registers across the MMA loop than pointers.
 struct PendingRelease {
-  uint64_t* bar0 = nullptr;
-  uint64_t* bar1 = nullptr;
+  uint32_t bar0 = 0;
+  uint32_t bar1 = 0;
   __device__ __forceinline__ void release(bool leader) {
     if (leader) {
-      if (bar0) mbar_arrive(bar0);
-      if (bar1) mbar_arrive(bar1);
+      if (bar0) mbar_arrive_at(bar0);
+      if (bar1) mbar_arrive_at(bar1);
     }
-    bar0 = bar1 = nullptr;
+    bar0 = bar1 = 0;
   }
 };
 

@@ -6,7 +6,10 @@
 //               Stride-2 convolutions use the tensor map's element strides.
 //   B operand:  bf16 weights [cout][tap][cin] through a 3-D map (chunk x 1 x BN).
 //   MMA:        wgmma, M = 128 pixels (TH x TW patch) split over two consumer warpgroups of 64 rows, N = BN <= 256,
-//               K = 16 per instruction, fp32 accumulators in registers.
+//               K = 16 per instruction, fp32 accumulators in registers. Instantiated per (OCC, NB16 = BN / 16): each
+//               MMA's width and accumulator offset are compile-time constants, and a stage's K steps (KC / 16) select
+//               one of three fully unrolled group bodies before the fence, so one group stays in flight under the
+//               next (wgmma_wait<1>); tests/test_conv_sass.py checks the compiled code.
 //   Epilogue:   conv_epi.cuh, from the registers; BatchNorm sums of the *stored* values kept per warp (fixed order).
 //   Schedule:   persistent CTAs, round-robin tiles; 288 threads: warps 0-7 consumers, warp 8 TMA producer.
 //   Launch:     programmatic dependent launch (launch.h): the prologue overlaps the previous kernel's tail.
@@ -20,6 +23,8 @@
 #include "conv_common.h"
 #include "bn_fold.cuh"
 #include "conv_epi.cuh"
+#include <type_traits>
+#include <utility>
 
 namespace b200seg {
 
@@ -32,7 +37,7 @@ struct ConvKParams {
   int tap_dh[9], tap_dw[9], tap_w[9];     // input offset and weight-tap index per filter tap
   int cchunks, KC, BN, n_tiles;
   int TH, TW, tiles_h, tiles_w, total_tiles;
-  int y_ld, out_fp32, has_bias, emit_stats, cout_pad, addend_ld;
+  int y_ld, out_fp32, emit_stats, cout_pad, addend_ld;
   int layout_type, sbo;
   int a_bytes, b_bytes, stage_bytes, nstages;
 };
@@ -41,13 +46,14 @@ constexpr int kThreads = 288;
 constexpr int kMaxStages = 8;
 constexpr size_t kHalfSmBudget = 115712;   // (228 KB - 2 x 1 KB reserved) / 2: two CTAs per SM (see conv3x3_halo.cu)
 
-// OCC: CTAs per SM; the two-per-SM build holds at most 128 accumulator columns (64 registers per consumer thread).
-template <int OCC>
+// OCC: CTAs per SM; NB16 = BN / 16: 16-column accumulator blocks of the Cout tile (the two-per-SM build exists for
+// NB16 <= 8: at most 128 accumulator columns, 64 registers per consumer thread).
+template <int OCC, int NB16>
 __global__ void __launch_bounds__(kThreads, OCC)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                  const ConvKParams p, void* __restrict__ y, const float* __restrict__ bias,
+                  const __grid_constant__ ConvKParams p, void* __restrict__ y, const float* __restrict__ bias,
                   float* __restrict__ stats_partials, const __nv_bfloat16* __restrict__ addend, const BnFoldDev fold) {
-  constexpr int NB = OCC == 2 ? 8 : 16;    // 16-column accumulator blocks
+  static_assert(NB16 >= 1 && NB16 <= (OCC == 2 ? 8 : 16), "accumulator columns exceed the register budget");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // carve: [stages][A|B] (1024-aligned) | barriers | ticket | stats[kStatSlots][2][cout_pad]
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -105,32 +111,45 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     // ------------------------------------------------------------------ consumers: MMA + epilogue
     const uint32_t g = warp >> 2;              // warpgroup: pixel rows 64g .. 64g + 63 of the tile
     const bool leader = (threadIdx.x & 127) == 0;
-    float* my_stats = s_stats + (size_t)warp * 2 * p.cout_pad;
     const uint64_t tmpl = make_smem_desc(0, 16, p.sbo, p.layout_type);
     const uint32_t s0 = smem_u32(stage_base);
+    const uint32_t full0 = smem_u32(full_bar), empty0 = smem_u32(empty_bar);
     const uint32_t a_off = g * (uint32_t)(p.a_bytes / 2);
     const uint32_t b64 = (uint32_t)(64 * p.KC * 2) >> 4;
-    const int ksteps = p.KC >> 4;
-    const int nb16 = p.BN >> 4;
-    ConvEpi e{y, p.has_bias ? bias : nullptr, addend, p.y_ld, p.addend_ld, p.out_fp32, p.Cout, p.emit_stats, p.cout_pad};
-    float acc[NB * 8];
     int stage = 0;
     uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      // Defined afresh per tile: the wgmma operands read the accumulators, so without this every accumulator of the
+      // previous tile would stay live through its whole epilogue (the first MMA of a tile uses scale-d 0 and ignores
+      // these zeros).
+      float acc[NB16 * 8];
+#pragma unroll
+      for (int i = 0; i < NB16 * 8; ++i) acc[i] = 0.f;
       PendingRelease pend;
       for (int kb = 0; kb < kblocks; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
+        mbar_wait_at(full0 + 8 * stage, phase);
         const uint32_t sa = s0 + (uint32_t)stage * (uint32_t)p.stage_bytes;
         const uint64_t adesc = tmpl + (uint64_t)((sa + a_off) >> 4);
         const uint64_t bdesc = tmpl + (uint64_t)((sa + (uint32_t)p.a_bytes) >> 4);
-        wgmma_fence();
-        // advancing K by 16 bf16 = 32 bytes inside the swizzle atom: +2 in the 16-byte-unit address field
-        for (int k = 0; k < ksteps; ++k)
-          wgmma_row<NB, 0, 0>(acc, nb16, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), b64, (kb | k) != 0);
-        wgmma_commit();
+        // One stage = KS = KC / 16 K steps, fully unrolled: nothing between the fence and the commit depends on a
+        // run-time value, so ptxas keeps the accumulators in registers and the group in flight.
+        auto stage_mma = [&](auto ks_const) {
+          constexpr int KS = decltype(ks_const)::value;
+          wgmma_fence();
+          // advancing K by 16 bf16 = 32 bytes inside the swizzle atom: +2 in the 16-byte-unit address field
+#pragma unroll
+          for (int k = 0; k < KS; ++k)
+            wgmma_row<NB16, 0, 0>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), b64, (kb | k) != 0);
+          wgmma_commit();
+        };
+        switch (p.KC >> 4) {
+          case 1: stage_mma(std::integral_constant<int, 1>()); break;
+          case 2: stage_mma(std::integral_constant<int, 2>()); break;
+          default: stage_mma(std::integral_constant<int, 4>()); break;
+        }
         wgmma_wait<1>();
         pend.release(leader);
-        pend.bar0 = &empty_bar[stage];
+        pend.bar0 = empty0 + 8 * stage;
         if (++stage == p.nstages) { stage = 0; phase ^= 1; }
       }
       wgmma_wait<0>();
@@ -153,7 +172,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const int ho = hs * p.out_stride + p.out_off_h, wo = ws * p.out_stride + p.out_off_w;
         pix[r] = ((size_t)img * p.Ho + ho) * p.Wo + wo;
       }
-      conv_epilogue<NB>(acc, nb16, n_tile * p.BN, valid, pix, e, fold, my_stats, lane);
+      const ConvEpi e{y, bias, addend, p.y_ld, p.addend_ld, p.out_fp32, p.Cout, p.emit_stats, p.cout_pad};
+      conv_epilogue<NB16>(acc, n_tile * p.BN, valid, pix, e, fold, smem_u32(s_stats) + warp * 8 * p.cout_pad, lane);
     }
   }
 
@@ -342,6 +362,27 @@ int make_bn_fold(const b200seg_bn_fold* f, int cout, BnFoldDev* out) {
   return 0;
 }
 
+// The instantiation of a launch: CTAs per SM (occ) and Cout tile width (nb16 = BN / 16).
+using IgemmKernel = void (*)(CUtensorMap, CUtensorMap, ConvKParams, void*, const float*, float*, const __nv_bfloat16*,
+                             BnFoldDev);
+template <int OCC, int... I>
+static IgemmKernel igemm_kernel_of(int nb16, std::integer_sequence<int, I...>) {
+  static constexpr IgemmKernel k[] = {conv_igemm_kernel<OCC, I + 1>...};
+  return k[nb16 - 1];
+}
+static IgemmKernel igemm_kernel(int occ, int nb16) {
+  return occ == 2 ? igemm_kernel_of<2>(nb16, std::make_integer_sequence<int, 8>())
+                  : igemm_kernel_of<1>(nb16, std::make_integer_sequence<int, 16>());
+}
+static cudaError_t igemm_set_attributes(IgemmKernel k, int occ) {
+  cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       occ == 2 ? (int)kHalfSmBudget : 227 * 1024);
+  // two CTAs per SM need (almost) the whole 228 KB as shared memory: ask for the maximum carve-out explicitly
+  if (e == cudaSuccess && occ == 2)
+    e = cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  return e;
+}
+
 static int launch_geom(const LaunchGeom& g, const void* a, const void* w, const float* bias, void* out,
                        float* stats_partials, int32_t* stats_grid, const void* addend, int addend_ld,
                        cudaStream_t stream, const b200seg_bn_fold* fold = nullptr, const BnFoldDev* affine = nullptr) {
@@ -387,54 +428,52 @@ static int launch_geom(const LaunchGeom& g, const void* a, const void* w, const 
   for (int t = 0; t < 9; ++t) { p.tap_dh[t] = g.tap_dh[t]; p.tap_dw[t] = g.tap_dw[t]; p.tap_w[t] = g.tap_w[t]; }
   p.cchunks = pl.cchunks; p.KC = pl.KC; p.BN = pl.BN; p.n_tiles = pl.n_tiles;
   p.TH = pl.TH; p.TW = pl.TW; p.tiles_h = pl.tiles_h; p.tiles_w = pl.tiles_w; p.total_tiles = pl.total_tiles;
-  p.y_ld = g.out_ld; p.out_fp32 = g.out_fp32; p.has_bias = g.has_bias; p.emit_stats = g.emit_stats;
+  p.y_ld = g.out_ld; p.out_fp32 = g.out_fp32; p.emit_stats = g.emit_stats;
   p.cout_pad = pl.cout_pad; p.addend_ld = addend_ld;
   p.layout_type = pl.KC == 64 ? 1 : (pl.KC == 32 ? 2 : 3);   // 128B / 64B / 32B swizzle
   p.sbo = 8 * pl.KC * 2;
   p.a_bytes = pl.a_bytes; p.b_bytes = pl.b_bytes; p.stage_bytes = pl.stage_bytes; p.nstages = pl.nstages;
 
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv_igemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  const IgemmKernel kernel = igemm_kernel(pl.occ, pl.BN / 16);
+  static bool attr_set[2][16] = {};
+  if (!attr_set[pl.occ - 1][pl.BN / 16 - 1]) {
+    cudaError_t e = igemm_set_attributes(kernel, pl.occ);
     if (e != cudaSuccess) return (int)e;
-    e = cudaFuncSetAttribute(conv_igemm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHalfSmBudget);
-    if (e != cudaSuccess) return (int)e;
-    // two CTAs per SM need (almost) the whole 228 KB as shared memory: ask for the maximum carve-out explicitly
-    e = cudaFuncSetAttribute(conv_igemm_kernel<2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    if (e != cudaSuccess) return (int)e;
-    attr_set = true;
+    attr_set[pl.occ - 1][pl.BN / 16 - 1] = true;
   }
   if (stats_grid) *stats_grid = pl.grid;
-  cudaError_t e =
-      pl.occ == 2 ? launch_k(conv_igemm_kernel<2>, dim3(pl.grid), dim3(kThreads), pl.smem_bytes, stream, tmA, tmB, p, out,
-                             bias, stats_partials, (const __nv_bfloat16*)addend, fd)
-                  : launch_k(conv_igemm_kernel<1>, dim3(pl.grid), dim3(kThreads), pl.smem_bytes, stream, tmA, tmB, p, out,
-                             bias, stats_partials, (const __nv_bfloat16*)addend, fd);
+  cudaError_t e = launch_k(kernel, dim3(pl.grid), dim3(kThreads), pl.smem_bytes, stream, tmA, tmB, p, out,
+                           g.has_bias ? bias : nullptr,
+                           stats_partials, (const __nv_bfloat16*)addend, fd);
   return e == cudaSuccess ? 0 : (int)e;
 }
 
+// CTAs per SM the runtime grants the widest Cout tile of the OCC build (NB16 = 8 / 16: the most accumulator registers)
 int conv_igemm_occupancy(int occ_variant, int smem_bytes) {
   int nb = -1;
-  cudaFuncSetAttribute(conv_igemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(conv_igemm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHalfSmBudget);
-  cudaFuncSetAttribute(conv_igemm_kernel<2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  cudaError_t e = occ_variant == 2
-      ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, conv_igemm_kernel<2>, kThreads, (size_t)smem_bytes)
-      : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, conv_igemm_kernel<1>, kThreads, (size_t)smem_bytes);
+  const IgemmKernel k = igemm_kernel(occ_variant, occ_variant == 2 ? 8 : 16);
+  igemm_set_attributes(k, occ_variant);
+  cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k, kThreads, (size_t)smem_bytes);
   return e == cudaSuccess ? nb : -(int)e;
 }
 
 void conv_igemm_occupancy_report() {
-  conv_igemm_occupancy(2, 1024);
-  for (int v = 2; v >= 1; --v) {
-    cudaFuncAttributes a;
-    if (v == 2) cudaFuncGetAttributes(&a, conv_igemm_kernel<2>); else cudaFuncGetAttributes(&a, conv_igemm_kernel<1>);
-    printf("conv_igemm_kernel<%d>: regs %d static smem %zu local %zu maxThreads %d maxDynSmem %d carveout %d\n  blocks/SM by dyn smem:",
-           v, a.numRegs, a.sharedSizeBytes, a.localSizeBytes, a.maxThreadsPerBlock, a.maxDynamicSharedSizeBytes,
-           a.preferredShmemCarveout);
-    for (int kb = 0; kb <= 112; kb += 16) printf(" %dK:%d", kb, conv_igemm_occupancy(v, kb * 1024));
-    printf("\n");
-  }
+  for (int v = 2; v >= 1; --v)
+    for (int nb16 = 1; nb16 <= (v == 2 ? 8 : 16); ++nb16) {
+      const IgemmKernel k = igemm_kernel(v, nb16);
+      igemm_set_attributes(k, v);
+      cudaFuncAttributes a;
+      cudaFuncGetAttributes(&a, k);
+      printf("conv_igemm_kernel<%d, %d>: regs %d static smem %zu local %zu maxThreads %d maxDynSmem %d carveout %d\n"
+             "  blocks/SM by dyn smem:", v, nb16, a.numRegs, a.sharedSizeBytes, a.localSizeBytes, a.maxThreadsPerBlock,
+             a.maxDynamicSharedSizeBytes, a.preferredShmemCarveout);
+      for (int kb = 0; kb <= 112; kb += 16) {
+        int nb = -1;
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k, kThreads, (size_t)kb * 1024);
+        printf(" %dK:%d", kb, nb);
+      }
+      printf("\n");
+    }
 }
 
 int conv3x3_halo_launch(int n, int h, int w, int cin, int in_ld, const void* in, int cout, const void* wts,

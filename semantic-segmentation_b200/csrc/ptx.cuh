@@ -48,23 +48,26 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
                : "memory");
 }
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t phase) {
+// barrier given by its shared-memory address (one 32-bit register instead of a generic pointer)
+__device__ __forceinline__ bool mbar_try_wait_at(uint32_t bar, uint32_t phase) {
   uint32_t ok;
   asm volatile(
       "{\n\t.reg .pred P;\n\t"
       "mbarrier.try_wait.parity.shared::cta.b64 P, [%1], %2;\n\t"
       "selp.u32 %0, 1, 0, P;\n\t}"
       : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(phase)
+      : "r"(bar), "r"(phase)
       : "memory");
   return ok != 0;
 }
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t phase) {
+__device__ __forceinline__ void mbar_wait_at(uint32_t bar, uint32_t phase) {
   uint32_t spins = 0;
-  while (!mbar_try_wait(bar, phase)) {
+  while (!mbar_try_wait_at(bar, phase)) {
     if (++spins > B200SEG_SPIN_LIMIT) __trap();
   }
 }
+__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t phase) { return mbar_try_wait_at(smem_u32(bar), phase); }
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t phase) { mbar_wait_at(smem_u32(bar), phase); }
 
 
 // ---------------------------------------------------------------- programmatic dependent launch (PDL)
@@ -132,6 +135,15 @@ __device__ __forceinline__ void tma_store_wait_all() {
 }
 __device__ __forceinline__ void named_barrier_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+// fp32 shared-memory load / store by 32-bit shared address (ordered with each other and with other memory accesses)
+__device__ __forceinline__ float ld_shared_f32(uint32_t addr) {
+  float v;
+  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_shared_f32(uint32_t addr, float v) {
+  asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
 }
 __device__ __forceinline__ void st_shared_v4(void* dst, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(smem_u32(dst)), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");

@@ -23,27 +23,29 @@ sys.path.insert(0, os.path.join(ROOT, "semantic-segmentation_b200"))
 PEAK_TFLOPS = 989.0   # H100 SXM, dense bf16, data sheet (700 W)
 
 
-def trace_launches(arch, height, width):
-    """[(ConvDesc field values, dy_ld, launches per step)] of the step's weight gradients (run under python -O)."""
-    from b200seg import _lib
+def record_calls(arch, height, width, key):
+    """Counter {key(name, args): calls per step} over the launching entry points of the traced step, for the calls whose
+    key is not None (tools/trace_step.py's recorder: meta tensors, no device; run under python -O)."""
     spec = importlib.util.spec_from_file_location("trace_step", os.path.join(ROOT, "tools", "trace_step.py"))
     ts = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(ts)
     seen = collections.Counter()
     base = ts.Recorder
 
-    class WgradRecorder(base):
+    class KeyRecorder(base):
         def __getattr__(self, name):
             fake = base.__getattr__(self, name)
-            if name != "b200seg_conv2d_wgrad":
+            if ts.QUERY.search(name):
                 return fake
 
-            def record(d, x, dy, dy_ld, *rest):
-                seen[(tuple(getattr(d._obj, f) for f, _ in _lib.ConvDesc._fields_), dy_ld)] += 1
-                return fake(d, x, dy, dy_ld, *rest)
+            def record(*args):
+                k = key(name, args, ts.SIZES)
+                if k is not None:
+                    seen[k] += 1
+                return fake(*args)
             return record
 
-    ts.Recorder = WgradRecorder
+    ts.Recorder = KeyRecorder
     argv, sys.argv = sys.argv, ["trace_step.py", "--arch", arch, "--height", str(height), "--width", str(width),
                                 "--bn-cells"]
     stdout, sys.stdout = sys.stdout, open(os.devnull, "w")
@@ -51,7 +53,44 @@ def trace_launches(arch, height, width):
         ts.main()
     finally:
         sys.stdout, sys.argv = stdout, argv
+    return seen
+
+
+def trace_launches(arch, height, width):
+    """[(ConvDesc field values, dy_ld, launches per step)] of the step's weight gradients (run under python -O)."""
+    from b200seg import _lib
+
+    def key(name, args, sizes):
+        if name != "b200seg_conv2d_wgrad":
+            return None
+        d, dy_ld = args[0]._obj, args[3]
+        return tuple(getattr(d, f) for f, _ in _lib.ConvDesc._fields_), dy_ld
+    seen = record_calls(arch, height, width, key)
     return [(list(desc), dy_ld, n) for (desc, dy_ld), n in seen.items()]
+
+
+def time_replay(launch, launches, reps):
+    """Microseconds per launch: CUDA events around a CUDA-graph replay of `launches` back-to-back calls of launch(),
+    after three eager calls and one warm-up replay; returns (median of `reps` replays, all replays)."""
+    import torch
+    for _ in range(3):
+        launch()
+    torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        for _ in range(launches):
+            launch()
+    g.replay()
+    torch.cuda.synchronize()
+    times = []
+    for _ in range(reps):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        g.replay()
+        e1.record()
+        torch.cuda.synchronize()
+        times.append(e0.elapsed_time(e1) * 1000.0 / launches)
+    return sorted(times)[len(times) // 2], times
 
 
 def card():
@@ -119,24 +158,7 @@ def main():
             if rc:
                 raise RuntimeError("b200seg_conv2d_wgrad returned %d for %s" % (rc, fields))
 
-        for _ in range(3):
-            launch()
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            for _ in range(args.launches):
-                launch()
-        g.replay()
-        torch.cuda.synchronize()
-        times = []
-        for _ in range(args.reps):
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            g.replay()
-            e1.record()
-            torch.cuda.synchronize()
-            times.append(e0.elapsed_time(e1) * 1000.0 / args.launches)
-        us = sorted(times)[len(times) // 2]
+        us, times = time_replay(launch, args.launches, args.reps)
         tflops = flop / us / 1e6
         label = "%dx%d c%d->%d k%d s%d" % (d.h, d.w, d.cin, d.cout, d.ksize, d.stride)
         print("%-34s %6d %-22s %9.1f %8.1f %6.1f%% %10.1f" % (label, count, "%d %d %d" % (plan[0], plan[2], plan[4]),
@@ -147,7 +169,7 @@ def main():
                          tflops=round(tflops, 1)))
         total_us += us * count
         total_flop += flop * count
-        del g, x, dy, dw, ws
+        del x, dy, dw, ws
     tflops = total_flop / total_us / 1e6
     print("per step: %d launches, %.3f TFLOP, %.3f ms, %.1f TFLOP/s (%.1f%% of 989)" %
           (sum(r["launches_per_step"] for r in rows), total_flop / 1e12, total_us / 1e3, tflops,
