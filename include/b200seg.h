@@ -87,15 +87,14 @@ size_t b200seg_conv2d_stats_elems(const b200seg_conv_desc* d);
 int b200seg_conv2d_fwd(const b200seg_conv_desc* d, const void* x, const void* w_ohwi, const float* bias, void* y,
                        float* stats_partials, int32_t* stats_grid, void* stream);
 
-/* The same convolution with the training-mode BatchNorm statistics FINALISED inside the launch (no partial table, no
- * bn_finalize launch): every CTA adds its per-channel sums to `accum` (fp64), the last CTA to finish writes
- * scale / shift / mean / invstd (and the batch statistics / running statistics exactly like b200seg_bn_finalize) and
- * clears `accum` / `counter` again. accum: [2][roundup16(cout)] fp64 and counter: uint32, both owned by the caller,
- * zero before the first use and private to one (layer, scale pass) - launches that share them must be stream ordered.
- * Per-GPU statistics only (SyncBN uses b200seg_conv2d_fwd + b200seg_bn_finalize, whose exchange needs its own kernel). */
+/* The same convolution with deferred training-mode BatchNorm statistics (no partial table, no bn_finalize launch):
+ * every CTA adds its per-channel (sum, sum of squares) to the cells `accum` (fp64 [2][roundup16(cout)], owned by the
+ * caller, zeroed once per step, private to one (layer, scale pass)). The launch reads only fold->accum and fold->c; the
+ * BatchNorm apply pass that consumes the layer (b200seg_bn_apply_cells, same fold) finalises the totals in its prologue,
+ * so no finaliser launch sits between the convolution and its consumer. Per-GPU statistics only (SyncBN uses
+ * b200seg_conv2d_fwd + b200seg_bn_finalize, whose exchange needs its own kernel). */
 typedef struct b200seg_bn_fold {
   double* accum;
-  uint32_t* counter;
   const float* gamma;            /* may be NULL (1) */
   const float* beta;             /* may be NULL (0) */
   float* scale;
@@ -112,11 +111,6 @@ typedef struct b200seg_bn_fold {
 int b200seg_conv2d_fwd_bn(const b200seg_conv_desc* d, const void* x, const void* w_ohwi, const float* bias, void* y,
                           const b200seg_bn_fold* fold, void* stream);
 
-/* Deferred variant (fold->counter == NULL; only accum and c are read): the launch adds its statistics to the cells and
- * nothing else - the BatchNorm apply pass that consumes the layer finalises them in its prologue (b200seg_bn_apply_cells),
- * so no finaliser launch and no last-CTA tail sits between the convolution and its consumer. The caller zeroes the cells
- * once per step. */
-
 /* The same with a residual addend: y = conv(x) (+ bias) + addend[n,ho,wo,cout] (bf16, pitch addend_ld); the statistics
  * are those of the stored sum (pre-activation residual networks: network/wider_resnet.py:170-183). bf16 output only. */
 int b200seg_conv2d_fwd_add(const b200seg_conv_desc* d, const void* x, const void* w_ohwi, const float* bias,
@@ -125,7 +119,7 @@ int b200seg_conv2d_fwd_add(const b200seg_conv_desc* d, const void* x, const void
 
 /* Evaluation mode: BatchNorm from running statistics, the residual sum and the ReLU folded into the convolution epilogue:
  *   y = relu?(conv(x) * scale[co] + shift[co] (+ addend[n,ho,wo,co]))      (network/hrnetv2.py:50-66,86-106 in one launch)
- * scale / shift: fp32 [cout] (b200seg_bn_eval_params; a convolution bias is folded into shift by the caller), bf16 output,
+ * scale / shift: fp32 [cout] (from the running statistics; a convolution bias is folded into shift by the caller), bf16 output,
  * d->has_bias = d->emit_stats = d->out_fp32 = 0. */
 int b200seg_conv2d_fwd_affine(const b200seg_conv_desc* d, const void* x, const void* w_ohwi, const float* scale,
                               const float* shift, int32_t relu, const void* addend, int32_t addend_ld, void* y,
@@ -260,17 +254,14 @@ int b200seg_accum_f32(float* dst, const float* src, int64_t n, void* stream);
  * 1 / world_size of the data-parallel average (network/__init__.py:38-39 apex DDP). */
 int b200seg_publish_grads(float* dst, const float* src, int64_t n, const float* scale_dev, float scale_const,
                           int32_t accumulate, void* stream);
-/* eval mode: scale/shift from running statistics */
-int b200seg_bn_eval_params(int32_t c, const float* gamma, const float* beta, float eps, const float* running_mean,
-                           const float* running_var, float* scale, float* shift, void* stream);
 /* z = relu?(y*scale + shift [+ res]) [* post_scale[n][c]]   (post_scale carries the Dropout2d mask/(1-p),
  * network/ocr_utils.py:146). npix = n*h*w, hw = h*w. */
 int b200seg_bn_apply(const void* y, int32_t y_ld, const float* scale, const float* shift, const void* res,
                      int32_t res_ld, const float* post_scale, int32_t relu, void* z, int32_t z_ld, int64_t npix,
                      int32_t hw, int32_t c, void* stream);
-/* The same pass as the consumer of a convolution launched in deferred mode (b200seg_conv2d_fwd_bn with counter == NULL):
- * every block derives scale / shift from f->accum (fp64 [2][roundup16(c)] sums), block 0 writes f->scale / shift / mean /
- * invstd (+ batch or running statistics exactly like b200seg_bn_finalize). f->counter is ignored. */
+/* The same pass as the consumer of a convolution launched with b200seg_conv2d_fwd_bn: every block derives scale / shift
+ * from f->accum (fp64 [2][roundup16(c)] sums), block 0 writes f->scale / shift / mean / invstd (+ batch or running
+ * statistics exactly like b200seg_bn_finalize). */
 int b200seg_bn_apply_cells(const void* y, int32_t y_ld, const b200seg_bn_fold* f, const void* res, int32_t res_ld,
                            const float* post_scale, int32_t relu, void* z, int32_t z_ld, int64_t npix, int32_t hw,
                            int32_t c, void* stream);
@@ -282,13 +273,6 @@ int b200seg_bn_bwd_reduce(const void* dz, int32_t dz_ld, const void* mask, int32
 /* dgamma += sum g*xhat, dbeta += sum g (accumulating), c1 = sum g / count, c2 = sum g*xhat / count */
 int b200seg_bn_bwd_finalize(const float* partials, int32_t grid, int32_t c, float count, float* dgamma, float* dbeta,
                             float* c1, float* c2, const b200seg_bn_sync* sync, void* stream);
-/* bn_bwd_reduce with the finalisation folded into the launch (per-GPU statistics; csrc/bn_fold.cuh pattern): CTAs add
- * their sums to accum ([2][c] fp64, zero between launches, private to one layer and scale pass), the last CTA adds
- * dgamma / dbeta, writes c1 = sum(g)/npix, c2 = sum(g*xhat)/npix and clears accum / counter. */
-int b200seg_bn_bwd_reduce_finalize(const void* dz, int32_t dz_ld, const void* mask, int32_t mask_ld,
-                                   const float* post_scale, const void* y, int32_t y_ld, const float* mean,
-                                   const float* invstd, int64_t npix, int32_t hw, int32_t c, double* accum,
-                                   uint32_t* counter, float* dgamma, float* dbeta, float* c1, float* c2, void* stream);
 /* dy = gamma*invstd*(g - c1 - xhat*c2); optionally g_out (=|+=) g for the residual / identity branch */
 int b200seg_bn_bwd_apply(const void* dz, int32_t dz_ld, const void* mask, int32_t mask_ld, const float* post_scale,
                          const void* y, int32_t y_ld, const float* mean, const float* invstd, const float* gamma,

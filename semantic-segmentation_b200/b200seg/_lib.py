@@ -49,7 +49,7 @@ class BnSync(ctypes.Structure):
 
 
 class BnFold(ctypes.Structure):
-    _fields_ = [("accum", c_void_p), ("counter", c_void_p), ("gamma", c_void_p), ("beta", c_void_p),
+    _fields_ = [("accum", c_void_p), ("gamma", c_void_p), ("beta", c_void_p),
                 ("scale", c_void_p), ("shift", c_void_p), ("mean", c_void_p), ("invstd", c_void_p),
                 ("batch_stats_out", c_void_p), ("running_mean", c_void_p), ("running_var", c_void_p),
                 ("num_batches_tracked", c_void_p), ("eps", c_float), ("momentum", c_float), ("count", c_float),
@@ -101,14 +101,11 @@ SIGNATURES = {
     "b200seg_publish_grads": (ctypes.c_int, [V, V, I64, V, F, I32, V]),
     "b200seg_sgd_chunk": (I32, []),
     "b200seg_sgd_step": (ctypes.c_int, [V, V, V, I32, F, F, F, F, I32, I32, V]),
-    "b200seg_bn_eval_params": (ctypes.c_int, [I32, V, V, F, V, V, V, V, V]),
     "b200seg_bn_apply": (ctypes.c_int, [V, I32, V, V, V, I32, V, I32, V, I32, I64, I32, I32, V]),
     "b200seg_bn_apply_cells": (ctypes.c_int, [V, I32, ctypes.POINTER(BnFold), V, I32, V, I32, V, I32, I64, I32, I32, V]),
     "b200seg_bn_bwd_grid": (I32, [I64, I32]),
     "b200seg_bn_bwd_reduce": (ctypes.c_int, [V, I32, V, I32, V, V, I32, V, V, I64, I32, I32, V, V]),
     "b200seg_bn_bwd_finalize": (ctypes.c_int, [V, I32, I32, F, V, V, V, V, ctypes.POINTER(BnSync), V]),
-    "b200seg_bn_bwd_reduce_finalize": (ctypes.c_int, [V, I32, V, I32, V, V, I32, V, V, I64, I32, I32, V, V, V, V, V, V,
-                                                      V]),
     "b200seg_bn_bwd_apply": (ctypes.c_int, [V, I32, V, I32, V, V, I32, V, V, V, V, V, V, I32, V, I32, I32, I64, I32,
                                             I32, V]),
     "b200seg_bn_bwd_cells": (ctypes.c_int, [V, I32, V, I32, V, V, I32, V, V, V, V, V, V, V, I32, V, I32, I32, I64, I32,

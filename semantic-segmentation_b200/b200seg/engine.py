@@ -7,9 +7,15 @@ Design notes
   * ``Act`` is an NHWC bf16 activation (possibly a channel-slice view of a wider buffer, so concat is a no-op).
     ``Act.grad`` accumulates in place: producers of a gradient either create it or pass the existing buffer as the
     kernel's addend.
-  * conv -> training BatchNorm -> (residual) -> ReLU is three passes: the wgmma conv emits the batch statistics from
-    its epilogue, ``bn_finalize`` turns them into scale/shift (+ running stats), ``bn_apply`` fuses affine, residual,
-    ReLU and the Dropout2d mask. The backward mirrors it (``bn_bwd`` = reduce + finalize + apply, then wgrad, dgrad).
+  * conv -> training BatchNorm -> (residual) -> ReLU: with per-GPU statistics (``bncells``) it is two passes - the
+    wgmma conv adds the batch statistics of its output to the layer's fp64 cells from its epilogue, and ``bn_apply``
+    turns them into scale/shift (+ running stats) in its prologue and fuses affine, residual, ReLU and the Dropout2d
+    mask. The backward mirrors it (``bn_bwd`` = reduce + apply, then wgrad, dgrad). SyncBN, fuse layers and
+    pre-activation BatchNorms put a separate finaliser in between: the conv writes a table of per-CTA partials,
+    ``bn_finalize`` turns them into scale/shift (exchanging them across GPUs under SyncBN), and ``bn_bwd`` is
+    reduce + finalize + apply.
+  * Evaluation takes scale/shift from the running statistics (``eval_bn``) and folds BatchNorm, residual and ReLU into
+    the convolution epilogue where it can.
 """
 import contextlib
 
@@ -46,7 +52,7 @@ class HeadRec:
 
 class Engine:
     def __init__(self, params, grads, packed, training, drop_mask=None, side_stream=None, bstat=None, stream=None,
-                 sync=None, pass_id=0, branch_streams=None, ws_holder=None, bnfold=None, bncells=None):
+                 sync=None, pass_id=0, branch_streams=None, ws_holder=None, bncells=None):
         """params: name -> tensor (weights, BN buffers); grads: name -> fp32 tensor accumulated into (training);
         packed: name -> (w_fwd, w_dgrad) bf16 operand caches; drop_mask: fp32 [N, mid] post-ReLU multiplier;
         bstat: BN layer name -> fp32 [2*C] slot receiving the batch [mean | unbiased var] (the running statistics are
@@ -54,11 +60,9 @@ class Engine:
         stream: the stream this engine's program is enqueued on when it runs concurrently with another engine (the
         low-resolution pass of the two-scale step), None = the caller's current stream;
         sync / pass_id: SyncBNContext (p2p.py) and this engine's pass index in its exchange table (data parallel);
-        bnfold: BN layer name -> (fp64 accumulator, int32 ticket) cells: the BatchNorm statistics are finalised inside
-        the convolution launch (raw.conv2d_fwd_bn) instead of by a bn_finalize launch (per-GPU statistics only);
         bncells: BN layer name -> (fp64 forward cells [2*roundup16(c)], fp64 backward cells [2*c]), all zero at the start
         of the step: deferred finalisation - the convolution / the backward reduction only add their sums to the cells
-        and the consuming apply pass folds them in its prologue (no finaliser launch on the chain; per-GPU statistics);
+        and the consuming apply pass folds them in its prologue (no finaliser launch on the chain; ignored with sync);
         branch_streams: up to three extra streams for the parallel branches of a HighResolutionModule (branch 0 stays
         on the engine's own stream); ws_holder: reusable weight-gradient slab workspace of the side stream."""
         self.p = params
@@ -72,13 +76,11 @@ class Engine:
         self.pass_id = pass_id
         self.bstreams = list(branch_streams or [])
         self.ws_holder = ws_holder
-        self.bnfold = bnfold if sync is None else None
-        self.bncells = bncells if (sync is None and self.bnfold is None) else None
+        self.bncells = bncells if sync is None else None
         self.eval_bn = None      # evaluation: BN layer name -> (scale, shift) from the running statistics (evalpath.py)
         self._ctx = None         # stream of the branch section being recorded (None = the engine's own stream)
         self.pre_backward_event = None   # e.g. "data-gradient weight operands packed" (recorded on another stream)
         self.tape = []
-        self.on_mark = None      # callable(engine, tag): fired in backward when everything recorded after mark(tag) has run
         self.bn_seen = set()
         self.hold = []      # tensors handed across streams: kept alive until the step's final join
         # Weight gradients do not feed the rest of the backward chain: they run on a side stream (a parallel branch of
@@ -101,9 +103,6 @@ class Engine:
                 else:
                     with torch.cuda.stream(st):
                         fn()
-            elif kind == "mark":
-                if self.on_mark is not None:
-                    self.on_mark(self, fn)
             elif kind == "join":          # forward joined k branches here: backward forks them
                 self._fork_streams(fn)
             else:                          # forward forked here: backward joins
@@ -152,13 +151,6 @@ class Engine:
         finally:
             self._ctx = prev
 
-    def mark(self, tag):
-        """Checkpoint on the main chain of the program: in backward, on_mark(self, tag) fires once the gradients of
-        everything recorded AFTER this point are enqueued (used to hand finished parameter-gradient buckets to the
-        data-parallel all-reduce while the rest of the backward still runs)."""
-        if self.training:
-            self.tape.append(("mark", tag, None))
-
     def finish(self):
         """After every stream of the step has been joined: drop the cross-stream keep-alive references."""
         self.hold.clear()
@@ -206,19 +198,7 @@ class Engine:
             par = rec.par = raw._new((4, rec.cout), dtype=F32, device=x.t.device)
             rec.scale, rec.shift, rec.mean, rec.invstd = par[0], par[1], par[2], par[3]
             return rec
-        if self.training and self.bnfold is not None:
-            acc, ticket = self.bnfold[bname]
-            if self.bstat is not None:
-                self.bn_seen.add(bname)
-                y, par = raw.conv2d_fwd_bn(x.t, w_f, b, stride, self.p[bname + ".weight"], self.p[bname + ".bias"], BN_EPS,
-                                           BN_MOMENTUM, acc, ticket, batch_out=self.bstat[bname], dilation=dilation)
-            else:
-                y, par = raw.conv2d_fwd_bn(x.t, w_f, b, stride, self.p[bname + ".weight"], self.p[bname + ".bias"], BN_EPS,
-                                           BN_MOMENTUM, acc, ticket, running_mean=self.p[bname + ".running_mean"],
-                                           running_var=self.p[bname + ".running_var"],
-                                           nbt=self.p[bname + ".num_batches_tracked"], dilation=dilation)
-            rec.scale, rec.shift, rec.mean, rec.invstd = par[0], par[1], par[2], par[3]
-        elif self.training:
+        if self.training:
             y, stats = raw.conv2d_fwd(x.t, w_f, b, stride=stride, emit_stats=True, dilation=dilation)
             n, ho, wo, _ = y.shape
             if self.bstat is not None:
@@ -233,9 +213,7 @@ class Engine:
             rec.scale, rec.shift, rec.mean, rec.invstd = par[0], par[1], par[2], par[3]
         else:
             y = raw.conv2d_fwd(x.t, w_f, b, stride=stride, dilation=dilation)
-            par = self.eval_bn[bname] if self.eval_bn is not None else raw.bn_eval_params(
-                self.p[bname + ".weight"], self.p[bname + ".bias"], BN_EPS, self.p[bname + ".running_mean"],
-                self.p[bname + ".running_var"])
+            par = self.eval_bn[bname]
             rec.scale, rec.shift, rec.mean, rec.invstd = par[0], par[1], None, None
         rec.y = y
         return rec
@@ -248,7 +226,6 @@ class Engine:
         dy = raw.bn_bwd(dz, mask, post_scale, rec.y, rec.mean, rec.invstd, self.p[rec.bname + ".weight"],
                         self.g[rec.bname + ".weight"], self.g[rec.bname + ".bias"], g_out=g_out,
                         g_accumulate=g_accumulate, sync=self._sync(rec.bname, 1),
-                        fold=self.bnfold[rec.bname] if self.bnfold is not None else None,
                         cells=self.bncells[rec.bname][1] if self.bncells is not None else None)
         x = rec.x
         self.wgrad(x.t, dy, self.g[rec.cname + ".weight"], rec.cout, rec.ksize, rec.stride, rec.dil)
@@ -294,7 +271,7 @@ class Engine:
 
     def conv_bn(self, x, cname, bname, ksize, stride=1, relu=True, residual=None, out=None, bias=False,
                 post_scale=None, dilation=1):
-        if not self.training and self.eval_bn is not None and post_scale is None:
+        if not self.training and post_scale is None:
             # evaluation: BatchNorm (running statistics), residual sum and ReLU in the convolution epilogue - one launch
             w_f, _ = self.packed[cname]
             scale, shift = self.eval_bn[bname]
@@ -360,11 +337,8 @@ class Engine:
             par = raw.bn_finalize(x.stats, n * h * w, self.p[bname + ".weight"], self.p[bname + ".bias"], BN_EPS,
                                   BN_MOMENTUM, self.p[bname + ".running_mean"], self.p[bname + ".running_var"],
                                   self.p[bname + ".num_batches_tracked"], c, sync=self._sync(bname, 0))
-        elif self.eval_bn is not None:
-            par = self.eval_bn[bname]
         else:
-            par = raw.bn_eval_params(self.p[bname + ".weight"], self.p[bname + ".bias"], BN_EPS,
-                                     self.p[bname + ".running_mean"], self.p[bname + ".running_var"])
+            par = self.eval_bn[bname]
         a = raw.bn_apply(x.t, par[0], par[1], None, post_scale, True)
         aa = Act(a)
 

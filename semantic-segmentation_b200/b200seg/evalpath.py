@@ -41,10 +41,8 @@ def eval_forward(module, images):
     tensors = {k: v.detach() for k, v in module._tensors().items()}
     E = Engine(tensors, {}, module._packed, False, None)
     # BatchNorm from running statistics: every layer's scale / shift up front; conv + BN (+ residual) + ReLU then run as
-    # ONE launch each (raw.conv2d_fwd_affine). B200SEG_EVAL_FUSED=0: separate bn_eval_params / bn_apply launches.
-    import os
-    if os.environ.get("B200SEG_EVAL_FUSED", "1") == "1":
-        E.eval_bn = module._eval_bn_params()
+    # ONE launch each (raw.conv2d_fwd_affine).
+    E.eval_bn = module._eval_bn_params()
     arch = module.arch
     if arch == "deepv3.DeepV3PlusW38":          # DeepV3Plus.forward eval branch (network/deepv3.py:73-96)
         head = M.deepv3_pass(E, images, module.hcfg)

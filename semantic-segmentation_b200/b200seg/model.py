@@ -72,8 +72,6 @@ def hrnet_forward(E, x16, hcfg, p="backbone"):
         sc = hcfg[key]
         ch = sc["num_channels"]
         tp = "%s.transition%d" % (p, si)
-        if key == "stage4":
-            E.mark("stage4")         # backward: the gradients of transition3 + stage4 are complete when this pops
         xs = []
         for i in range(len(ch)):
             if i < len(pre):
@@ -301,7 +299,6 @@ def scale_pass(E, images, size_hw, arch, hcfg, ocfg):
     blend/loss kernels). images: fp32 NCHW; size_hw: pass input size (ResizeX folded into image_prep)."""
     x16 = Act(raw.image_prep(images, size_hw[0], size_hw[1]), needs_grad=False)
     feats = hrnet_forward(E, x16, hcfg)
-    E.mark("heads")                  # backward: the gradients of every head parameter are complete when this pops
     if arch == "basic.HRNet":
         return dict(cls=seg_head(E, feats), aux=None, attn=None)
     if arch == "mscale.HRNet":      # MscaleBasic._fwd (network/mscale.py:463-470): both heads read the trunk features

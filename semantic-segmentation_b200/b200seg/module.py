@@ -133,16 +133,6 @@ class B200SegModule(nn.Module):
         # NVLink peer memory (needs torch.distributed, world > 1); None / False = per-GPU statistics. Opt-in for now: the
         # exchange was validated on 2 GPUs only.
         self.syncbn = syncbn
-        # BatchNorm statistics finalised inside the producing launches (csrc/bn_fold.cuh): 1262 launches fewer per step,
-        # but measured 0.9 ms SLOWER on the device (40.18 vs 39.3 ms, alternating runs on one box: the tail of every
-        # convolution grows by ~4 us while the removed finalisers ran on a handful of SMs next to other work) with no
-        # clear end-to-end gain, so it is opt-in (B200SEG_FUSED_BN=1); SyncBN always uses the separate finaliser.
-        import os
-        self.fused_bn_finalize = os.environ.get("B200SEG_FUSED_BN", "0") == "1"
-        # Deferred finalisation (default): the convolution / the backward reduction add their sums to per-layer fp64
-        # cells and the consuming apply pass folds them in its prologue - no finaliser launch and no last-CTA tail on
-        # the chain conv -> BN -> conv (B200SEG_BN_CELLS=0: separate bn_finalize / bn_bwd_finalize launches).
-        self.bn_cells = os.environ.get("B200SEG_BN_CELLS", "1") == "1" and not self.fused_bn_finalize
         self._sync = None
         self._run_flat = None
         self._specs = A.tensor_specs(arch, self.hcfg, self.ocfg)
@@ -274,18 +264,6 @@ class B200SegModule(nn.Module):
                 segs.append((off, off, 1, numel, 1, numel))
             off += (numel + 63) // 64 * 64
         self._fold_table = raw.grad_fold_table(segs, dev)
-        # Gradient buckets for the overlapped data-parallel all-reduce, contiguous in the flat layout (= registration
-        # order) and listed in the order the backward completes them: heads, transition3 + stage4, everything before.
-        names = [n for n, _ in params]
-        i1 = next((i for i, n in enumerate(names) if n.startswith("backbone.transition3.")), 0)
-        i2 = next((i for i, n in enumerate(names) if not n.startswith("backbone.")), len(names))
-        i1 = min(i1, i2)
-        self._buckets = []
-        for tag, (a, b) in (("heads", (i2, len(names))), ("stage4", (i1, i2)), ("rest", (0, i1))):
-            if b > a:
-                lo = segs[a][0]
-                hi = segs[b - 1][0] + (segs[b - 1][2] * segs[b - 1][3] * segs[b - 1][4] + 63) // 64 * 64
-                self._buckets.append(dict(tag=tag, lo=lo, hi=hi, table=raw.grad_fold_table(segs[a:b], dev)))
 
     def _engine_grads(self, which="hi"):
         """name -> fp32 tensor an Engine accumulates into."""
@@ -326,20 +304,7 @@ class B200SegModule(nn.Module):
                 self._bn_slots[b] = (off, c)
                 off += 2 * c
         self._run_flat, self._nbt_flat = flat, nbt_flat
-        # self-clearing reduction cells of the in-launch BatchNorm finalisation (raw.conv2d_fwd_bn), one set per pass
-        self._bnfold = []
-        for _pass in range(2):
-            cells = {}
-            acc = torch.zeros(sum(2 * ((c_ + 15) // 16 * 16) for _o, c_ in self._bn_slots.values()), dtype=torch.float64,
-                              device=dev)
-            tickets = torch.zeros(len(self._bn_slots), dtype=torch.int32, device=dev)
-            o = 0
-            for li, (b, (_o, c_)) in enumerate(self._bn_slots.items()):
-                cp = (c_ + 15) // 16 * 16
-                cells[b] = (acc[o:o + 2 * cp], tickets[li:li + 1])
-                o += 2 * cp
-            self._bnfold.append(cells)
-        # deferred BatchNorm finalisation (csrc/bn_fold.cuh, counter == NULL): per pass and layer a forward cell pair
+        # deferred BatchNorm finalisation (csrc/bn_fold.cuh): per pass and layer a forward cell pair
         # [2 * roundup16(c)] and a backward one [2 * c], one fp64 arena zeroed at the start of every step
         n_cells = sum(2 * ((c_ + 15) // 16 * 16) + 2 * c_ for _o, c_ in self._bn_slots.values())
         self._bncell_arena = torch.zeros(2 * n_cells, dtype=torch.float64, device=dev)
@@ -358,7 +323,7 @@ class B200SegModule(nn.Module):
 
     def _eval_bn_params(self):
         """Evaluation: scale / shift of EVERY BatchNorm layer from the running statistics in a handful of launches
-        (instead of one bn_eval_params launch per layer and pass): name -> (scale, shift) fp32 views."""
+        (instead of one per layer and pass): name -> (scale, shift) fp32 views."""
         dev = self._run_flat.device
         names = list(self._bn_slots)
         if getattr(self, "_eval_idx", None) is None or self._eval_idx[0].device != dev:
@@ -406,28 +371,10 @@ class B200SegModule(nn.Module):
         from . import _lib
         launches0 = _lib.KERNEL_LAUNCHES
         try:
-            if not self._prio():
-                return self._step_body(images, gts, drop_mask)
-            # B200SEG_PRIO=1 (experiment): the scale passes and their branch streams run on high-priority streams, the
-            # weight-gradient / repack side streams (which feed nothing downstream inside the step) stay at the default
-            # priority; kernel-node priorities are captured into the graph
-            if getattr(self, "_prio_stream", None) is None:
-                self._prio_stream = torch.cuda.Stream(priority=-1)
-            cur = torch.cuda.current_stream()
-            self._prio_stream.wait_stream(cur)
-            with torch.cuda.stream(self._prio_stream):
-                loss = self._step_body(images, gts, drop_mask)
-            cur.wait_stream(self._prio_stream)
-            loss.record_stream(cur)
-            return loss
+            return self._step_body(images, gts, drop_mask)
         finally:
             raw.KEEP = None
             self.kernels_per_step = _lib.KERNEL_LAUNCHES - launches0   # same count when the captured graph replays
-
-    @staticmethod
-    def _prio():
-        import os
-        return os.environ.get("B200SEG_PRIO", "0") == "1"
 
     def _sync_context(self):
         """Lazily builds the SyncBN mailboxes (collective: every rank must reach its first training step)."""
@@ -447,43 +394,37 @@ class B200SegModule(nn.Module):
         if getattr(self, "_side_stream", None) is None:
             self._side_stream = torch.cuda.Stream()
         sync = self._sync
-        # SyncBN: B200SEG_SYNCBN_BRANCH_STREAMS=0 restores the two-chain structure (one stream per scale pass + its side
-        # stream, repack on the main stream); the default runs the same 21-stream program as per-GPU statistics - the
-        # one-warp waiter kernels never keep another kernel from being scheduled (csrc/bn_kernels.cu), so up to eight
-        # exchanges (four branches x two passes) are in flight and hide each other's NVLink round trips.
-        import os
-        wide = sync is None or os.environ.get("B200SEG_SYNCBN_BRANCH_STREAMS", "1") != "0"
-        wd_ready = self._repack(side=self._side_stream if wide else None)
+        # SyncBN runs the same 21-stream program as per-GPU statistics: the one-warp waiter kernels never keep another
+        # kernel from being scheduled (csrc/bn_kernels.cu), so up to eight exchanges (four branches x two passes) are in
+        # flight and hide each other's NVLink round trips.
+        wd_ready = self._repack(side=self._side_stream)
         if sync is not None:
             sync.advance()
         tensors = {k: v.detach() for k, v in self._tensors().items()}
         par = self.parallel_scales and A.is_two_scale(self.arch)
         # (one engine per scale pass, or a single pass: a layer's cells are used once per step)
-        use_cells = self.bn_cells and sync is None and (par or not A.is_two_scale(self.arch))
+        use_cells = sync is None and (par or not A.is_two_scale(self.arch))
         if use_cells:
             self._bncell_arena.zero_()
         self._acc_hi.zero_()         # two memsets (45 us each) beat clearing inside the fold's transposed gather
         if par:
             self._acc_lo.zero_()
         # every allocation of the step stays referenced until its final join (raw.py)
-        raw.KEEP = [] if wide else None
+        raw.KEEP = []
         if getattr(self, "_bstreams", None) is None:
-            use_b = self.parallel_branches and wide
-            pr = -1 if self._prio() else 0
-            mk = lambda: [torch.cuda.Stream(priority=pr) for _ in range(3)] if use_b else []
+            mk = lambda: [torch.cuda.Stream() for _ in range(3)] if self.parallel_branches else []
             self._bstreams = {"hi": mk(), "lo": mk()}
-            self._ws_holders = {"hi": [None] if wide else None, "lo": [None] if wide else None}
+            self._ws_holders = {"hi": [None], "lo": [None]}
         grads = self._engine_grads("hi")
         E_lo = None
         if par:
             if getattr(self, "_lo_stream", None) is None:
-                self._lo_stream = torch.cuda.Stream(priority=-1 if self._prio() else 0)
+                self._lo_stream = torch.cuda.Stream()
                 self._side_stream_lo = torch.cuda.Stream()
             grads_lo = self._engine_grads("lo")
             E_lo = Engine(tensors, grads_lo, self._packed, True, drop_mask, side_stream=self._side_stream_lo,
                           bstat=self._bstat_views[0], stream=self._lo_stream, sync=sync, pass_id=0,
                           branch_streams=self._bstreams["lo"], ws_holder=self._ws_holders["lo"],
-                          bnfold=self._bnfold[0] if self.fused_bn_finalize else None,
                           bncells=self._bncells[0] if use_cells else None)
         two_pass = A.is_two_scale(self.arch)
         if sync is not None and two_pass and not par:
@@ -491,7 +432,6 @@ class B200SegModule(nn.Module):
         E = Engine(tensors, grads, self._packed, True, drop_mask, side_stream=self._side_stream,
                    bstat=self._bstat_views[1] if par else None, sync=sync, pass_id=1 if two_pass else 0,
                    branch_streams=self._bstreams["hi"], ws_holder=self._ws_holders["hi"],
-                   bnfold=self._bnfold[1] if self.fused_bn_finalize else None,
                    bncells=self._bncells[1] if use_cells else None)
         loss = M.train_loss(E, images, gts, self.arch, self.hcfg, self.ocfg, self.lo_scale, self.ocr_alpha, self.sup_wt,
                             self.ignore_index, E_lo=E_lo, loss_kind=self.loss_kind, img_wt=self.img_wt,
@@ -499,74 +439,13 @@ class B200SegModule(nn.Module):
         E.pre_backward_event = wd_ready
         if E_lo is not None:
             E_lo.pre_backward_event = wd_ready
-        bucketed = self._bucketed_allreduce()
-        self._reduced_in_step = bucketed
-        if bucketed:
-            self._run_backward_bucketed(E, E_lo, par)
-        else:
-            M.run_backward(E, E_lo)
-            self._fold_grads(par)
+        M.run_backward(E, E_lo)
+        self._fold_grads(par)
         if par:
             assert E.bn_seen == E_lo.bn_seen and len(E.bn_seen) == len(self._bn_slots), "BN bookkeeping out of sync"
             raw.bn_running_update(self._run_flat, self._bstat[0], self._bstat[1], BN_MOMENTUM, self._nbt_flat, 2)
         raw.KEEP = None
         return loss
-
-    def _bucketed_allreduce(self):
-        """Data-parallel step: fold and all-reduce finished gradient buckets while the backward still runs."""
-        import os
-        # Opt-in (B200SEG_BUCKET_ALLREDUCE=1): NCCL's kernels wait for their peers while holding whole SMs, and every
-        # persistent convolution CTA owns its tiles statically - a convolution that shares the GPU with an all-reduce
-        # stalls until the collective leaves its SMs, and under SyncBN (compute that waits for the peer's compute) the
-        # combination can deadlock, so SyncBN mode never overlaps. Default: one all-reduce at gradient-publish time.
-        if not self._ddp_allreduce or self._sync is not None or os.environ.get("B200SEG_BUCKET_ALLREDUCE", "0") != "1":
-            return False
-        d = torch.distributed
-        return d.is_available() and d.is_initialized() and d.get_world_size() > 1
-
-    def _run_backward_bucketed(self, E, E_lo, par):
-        """Collective C1 overlapped with the backward (the reference's apex DDP overlaps its buckets the same way,
-        network/__init__.py:38-39): when the tapes of all scale passes have passed a bucket's marker, a communication
-        stream folds that bucket's accumulators into the step gradient (OIHW) and NCCL all-reduces its slice, while the
-        compute streams continue with the earlier layers. Inside the captured graph this is a side branch that joins at
-        the end of the step; the 1 / world_size average is applied by the publish kernel."""
-        if getattr(self, "_comm_stream", None) is None:
-            self._comm_stream = torch.cuda.Stream()
-        comm = self._comm_stream
-        engines = [E] + ([E_lo] if E_lo is not None else [])
-        seen = {}
-        works = []
-        by_tag = {b["tag"]: b for b in self._buckets}
-
-        def launch(bucket, events):
-            with torch.cuda.stream(comm):
-                for ev in events:
-                    comm.wait_event(ev)
-                raw.grad_fold(self._step_flat, self._acc_hi, self._acc_lo if par else None, bucket["table"], clear=False,
-                              overwrite=True)
-                works.append(torch.distributed.all_reduce(self._step_flat[bucket["lo"]:bucket["hi"]], async_op=True))
-
-        def on_mark(eng, tag):
-            if tag not in by_tag:
-                return
-            cur = torch.cuda.current_stream()
-            evs = [cur.record_event()]
-            if eng.side is not None:
-                evs.append(eng.side.record_event())
-            seen.setdefault(tag, []).extend(evs)
-            seen[tag + "#n"] = seen.get(tag + "#n", 0) + 1
-            if seen[tag + "#n"] == len(engines):
-                launch(by_tag[tag], seen[tag])
-
-        for eng in engines:
-            eng.on_mark = on_mark
-        M.run_backward(E, E_lo)                      # joins every compute stream on the current one at its end
-        if "rest" in by_tag:
-            launch(by_tag["rest"], [torch.cuda.current_stream().record_event()])
-        with torch.cuda.stream(comm):
-            for w in works:
-                w.wait()
-        torch.cuda.current_stream().wait_stream(comm)
 
     def _drop_mask(self, n, device):
         """Dropout2d(0.05) channel mask (network/ocr_utils.py:146) drawn from torch's generator, folded with 1/(1-p)."""
@@ -625,10 +504,7 @@ class B200SegModule(nn.Module):
         is a view of ONE flat fp32 buffer (what FusedSGD and the all-reduce work on)."""
         scale = 1.0
         if self._ddp_allreduce:
-            if getattr(self, "_reduced_in_step", False):       # the step all-reduced its buckets while it ran
-                scale = 1.0 / torch.distributed.get_world_size()
-            else:
-                scale = 1.0 / allreduce_sum_(self._step_flat)
+            scale = 1.0 / allreduce_sum_(self._step_flat)
         if grad_out is not None:
             grad_out = grad_out.detach().reshape(()).to(F32)
         params = list(self.named_parameters())

@@ -155,34 +155,6 @@ def conv2d_fwd(x, w_ohwi, bias=None, stride=1, out=None, out_fp32=False, emit_st
     return out
 
 
-def conv2d_fwd_bn(x, w_ohwi, bias, stride, gamma, beta, eps, momentum, accum, counter, batch_out=None,
-                  running_mean=None, running_var=None, nbt=None, out=None, dilation=1):
-    """Convolution + training-mode BatchNorm statistics finalised inside the launch (b200seg_conv2d_fwd_bn): returns
-    (y, params fp32 [4, cout] = scale, shift, mean, invstd). accum (fp64 [2*roundup16(cout)]) / counter (int32 [1]) are
-    the layer's private, self-clearing reduction cells."""
-    assert x.is_cuda and x.dtype == BF16
-    cout, taps, cin = w_ohwi.shape
-    assert cin == x.shape[3], (cin, x.shape)
-    ksize = 3 if taps == 9 else 1
-    n, h, w, _ = x.shape
-    ho, wo = out_hw(h, w, ksize, stride, dilation)
-    if out is None:
-        out = _new((n, ho, wo, cout), dtype=BF16, device=x.device)
-    d = conv_desc(n, h, w, cin, cout, ksize, stride, _ld(x), _ld(out), False, bias is not None, True,
-                  dilation=dilation)
-    par = _new((4, cout), dtype=F32, device=x.device)
-    f = BnFold()
-    f.accum, f.counter = ptr(accum), ptr(counter)
-    f.gamma, f.beta = ptr(gamma), ptr(beta)
-    f.scale, f.shift, f.mean, f.invstd = ptr(par[0]), ptr(par[1]), ptr(par[2]), ptr(par[3])
-    f.batch_stats_out = ptr(batch_out)
-    f.running_mean, f.running_var, f.num_batches_tracked = ptr(running_mean), ptr(running_var), ptr(nbt)
-    f.eps, f.momentum, f.count, f.c = eps, momentum, float(n * ho * wo), cout
-    check(lib().b200seg_conv2d_fwd_bn(ctypes.byref(d), ptr(x), ptr(w_ohwi), ptr(bias), ptr(out), ctypes.byref(f),
-                                      stream_ptr()), "conv2d_fwd_bn")
-    return out, par
-
-
 def conv2d_fwd_affine(x, w_ohwi, scale, shift, relu, stride=1, addend=None, out=None, dilation=1):
     """Evaluation: y = relu?(conv(x) * scale + shift (+ addend)) in one launch (BatchNorm from running statistics)."""
     assert x.is_cuda and x.dtype == BF16
@@ -202,7 +174,7 @@ def conv2d_fwd_affine(x, w_ohwi, scale, shift, relu, stride=1, addend=None, out=
 
 def _cells_fold(cells, par, gamma, beta, eps, momentum, count, c, batch_out, running_mean, running_var, nbt):
     f = BnFold()
-    f.accum, f.counter = ptr(cells), None          # counter NULL = deferred finalisation (csrc/bn_fold.cuh)
+    f.accum = ptr(cells)
     f.gamma, f.beta = ptr(gamma), ptr(beta)
     f.scale, f.shift, f.mean, f.invstd = ptr(par[0]), ptr(par[1]), ptr(par[2]), ptr(par[3])
     f.batch_stats_out = ptr(batch_out)
@@ -225,7 +197,7 @@ def conv2d_fwd_cells(x, w_ohwi, bias, stride, cells, out=None, dilation=1):
     d = conv_desc(n, h, w, cin, cout, ksize, stride, _ld(x), _ld(out), False, bias is not None, True,
                   dilation=dilation)
     f = BnFold()
-    f.accum, f.counter, f.c = ptr(cells), None, cout
+    f.accum, f.c = ptr(cells), cout
     check(lib().b200seg_conv2d_fwd_bn(ctypes.byref(d), ptr(x), ptr(w_ohwi), ptr(bias), ptr(out), ctypes.byref(f),
                                       stream_ptr()), "conv2d_fwd_bn(cells)")
     return out
@@ -352,14 +324,6 @@ def accum_f32(dst, src):
     check(lib().b200seg_accum_f32(ptr(dst), ptr(src), dst.numel(), stream_ptr()), "accum_f32")
 
 
-def bn_eval_params(gamma, beta, eps, running_mean, running_var):
-    c = gamma.shape[0]
-    out = _new((2, c), dtype=F32, device=gamma.device)
-    check(lib().b200seg_bn_eval_params(c, ptr(gamma), ptr(beta), eps, ptr(running_mean), ptr(running_var), ptr(out[0]),
-                                       ptr(out[1]), stream_ptr()), "bn_eval_params")
-    return out
-
-
 def bn_apply(y, scale, shift, res=None, post_scale=None, relu=True, out=None):
     n, h, w, c = y.shape
     if out is None:
@@ -371,10 +335,9 @@ def bn_apply(y, scale, shift, res=None, post_scale=None, relu=True, out=None):
 
 
 def bn_bwd(dz, mask, post_scale, y, mean, invstd, gamma, dgamma, dbeta, g_out=None, g_accumulate=False, dy_out=None,
-           sync=None, fold=None, cells=None):
-    """Returns dy (gradient w.r.t. the BN input). dgamma/dbeta (fp32 views) are accumulated into. fold = (fp64
-    accumulator [2*c], int32 ticket): finalise inside the reduce launch (per-GPU statistics, no bn_bwd_finalize).
-    cells (fp64 [2*c], zero at the start of the step): deferred finalisation inside the gradient pass (two launches)."""
+           sync=None, cells=None):
+    """Returns dy (gradient w.r.t. the BN input). dgamma/dbeta (fp32 views) are accumulated into. cells (fp64 [2*c],
+    zero at the start of the step): deferred finalisation inside the gradient pass (two launches, per-GPU statistics)."""
     n, h, w, c = y.shape
     npix = n * h * w
     L = lib()
@@ -386,19 +349,13 @@ def bn_bwd(dz, mask, post_scale, y, mean, invstd, gamma, dgamma, dbeta, g_out=No
                                      int(g_accumulate), npix, h * w, c, stream_ptr()), "bn_bwd_cells", launches=2)
         return dy
     cc = _new((2, c), dtype=F32, device=y.device)
-    if fold is not None and sync is None:
-        check(L.b200seg_bn_bwd_reduce_finalize(ptr(dz), _ld(dz), ptr(mask), _ld(mask) if mask is not None else 0,
-                                               ptr(post_scale), ptr(y), _ld(y), ptr(mean), ptr(invstd), npix, h * w, c,
-                                               ptr(fold[0]), ptr(fold[1]), ptr(dgamma), ptr(dbeta), ptr(cc[0]),
-                                               ptr(cc[1]), stream_ptr()), "bn_bwd_reduce_finalize")
-    else:
-        grid = L.b200seg_bn_bwd_grid(npix, c)
-        partials = _new((grid, 2, c), dtype=F32, device=y.device)
-        check(L.b200seg_bn_bwd_reduce(ptr(dz), _ld(dz), ptr(mask), _ld(mask) if mask is not None else 0,
-                                      ptr(post_scale), ptr(y), _ld(y), ptr(mean), ptr(invstd), npix, h * w, c,
-                                      ptr(partials), stream_ptr()), "bn_bwd_reduce")
-        check(L.b200seg_bn_bwd_finalize(ptr(partials), grid, c, float(npix), ptr(dgamma), ptr(dbeta), ptr(cc[0]),
-                                        ptr(cc[1]), _sync_ref(sync), stream_ptr()), "bn_bwd_finalize")
+    grid = L.b200seg_bn_bwd_grid(npix, c)
+    partials = _new((grid, 2, c), dtype=F32, device=y.device)
+    check(L.b200seg_bn_bwd_reduce(ptr(dz), _ld(dz), ptr(mask), _ld(mask) if mask is not None else 0,
+                                  ptr(post_scale), ptr(y), _ld(y), ptr(mean), ptr(invstd), npix, h * w, c,
+                                  ptr(partials), stream_ptr()), "bn_bwd_reduce")
+    check(L.b200seg_bn_bwd_finalize(ptr(partials), grid, c, float(npix), ptr(dgamma), ptr(dbeta), ptr(cc[0]),
+                                    ptr(cc[1]), _sync_ref(sync), stream_ptr()), "bn_bwd_finalize")
     dy = dy_out if dy_out is not None else _new((n, h, w, c), dtype=BF16, device=y.device)
     check(L.b200seg_bn_bwd_apply(ptr(dz), _ld(dz), ptr(mask), _ld(mask) if mask is not None else 0, ptr(post_scale),
                                  ptr(y), _ld(y), ptr(mean), ptr(invstd), ptr(gamma), ptr(cc[0]), ptr(cc[1]), ptr(dy),

@@ -275,20 +275,7 @@ __global__ void accum_f32_kernel(float* __restrict__ dst, const float* __restric
   }
 }
 
-// Eval-mode: scale/shift from the running statistics.
-__global__ void bn_eval_params_kernel(int C, const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
-                                      const float* __restrict__ running_mean, const float* __restrict__ running_var,
-                                      float* __restrict__ scale, float* __restrict__ shift) {
-  pdl_sync();
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
-  const float invstd = rsqrtf(running_var[c] + eps);
-  const float g_ = gamma[c];
-  scale[c] = g_ * invstd;
-  shift[c] = beta[c] - running_mean[c] * g_ * invstd;
-}
-
-// Deferred finalisation of the producing convolution's statistics (bn_fold.cuh, counter == nullptr): every block of the
+// Deferred finalisation of the producing convolution's statistics (bn_fold.cuh): every block of the
 // apply pass turns the fp64 totals into scale / shift for itself; block 0 also publishes the layer's parameters (the
 // backward pass reads mean / invstd, fuse layers scale / shift) and the batch / running statistics. cells == nullptr:
 // scale / shift come from bn_finalize (SyncBN, evaluation, statistics that did not come from a convolution epilogue).
@@ -381,22 +368,14 @@ bn_apply_kernel(const __nv_bfloat16* __restrict__ y, int y_ld, float* __restrict
 }
 
 // ------------------------------------------------------------------------------------------------ backward
-struct BnBwdFold {          // in-launch finalisation of bn_bwd_reduce (accum == nullptr: partial table + bn_bwd_finalize)
-  double* accum;            // [2][C] fp64, zero between launches
-  unsigned* counter;
-  float* dgamma;
-  float* dbeta;
-  float* c1;
-  float* c2;
-  float count;
-};
-
-// Thread (r, cg): r-th pixel row of the block, 8-channel group cg. blockDim.x = groups * rows.
+// Thread (r, cg): r-th pixel row of the block, 8-channel group cg. blockDim.x = groups * rows. The block's sums go to
+// `cells` ([2][C] fp64, added; bn_bwd_apply folds them) or, when cells == nullptr, to its row of `partials`
+// (bn_bwd_finalize folds them).
 __global__ void __launch_bounds__(256)
 bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ dz, int dz_ld, const __nv_bfloat16* __restrict__ mask,
                      int mask_ld, const float* __restrict__ post_scale, const __nv_bfloat16* __restrict__ y, int y_ld,
                      const float* __restrict__ mean, const float* __restrict__ invstd, long long npix, int hw, int C,
-                     int rows, float* __restrict__ partials, const BnBwdFold fold) {
+                     int rows, float* __restrict__ partials, double* __restrict__ cells) {
   pdl_sync();
   extern __shared__ float s_red[];   // [rows][groups][16]
   const int groups = C >> 3;
@@ -456,29 +435,9 @@ bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ dz, int dz_ld, const __nv
     float acc = 0.f;
     for (int rr = 0; rr < rows; ++rr) acc += s_red[((size_t)rr * groups + g_) * 16 + k];
     const int c = g_ * 8 + (k & 7);
-    if (fold.accum != nullptr) atomicAdd(fold.accum + (k >> 3) * C + c, (double)acc);
+    if (cells != nullptr) atomicAdd(cells + (k >> 3) * C + c, (double)acc);
     else partials[(size_t)blockIdx.x * 2 * C + (k >> 3) * C + c] = acc;
   }
-  if (fold.accum == nullptr || fold.counter == nullptr) return;   // counter == nullptr: bn_bwd_apply folds the cells
-  // In-launch finalisation (per-GPU statistics): the last CTA to finish turns the fp64 totals into dgamma / dbeta
-  // (accumulated) and the two mean terms of the input gradient, and clears the cells (see bn_fold.cuh for the pattern).
-  __shared__ unsigned s_ticket;
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) s_ticket = atomicAdd(fold.counter, 1u);
-  __syncthreads();
-  if (s_ticket != gridDim.x - 1) return;
-  __threadfence();
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    const double s1 = __ldcg(fold.accum + c), s2 = __ldcg(fold.accum + C + c);
-    fold.accum[c] = 0.0;
-    fold.accum[C + c] = 0.0;
-    if (fold.dbeta) fold.dbeta[c] += (float)s1;
-    if (fold.dgamma) fold.dgamma[c] += (float)s2;
-    fold.c1[c] = (float)(s1 / (double)fold.count);
-    fold.c2[c] = (float)(s2 / (double)fold.count);
-  }
-  if (threadIdx.x == 0) *fold.counter = 0u;
 }
 
 __global__ void __launch_bounds__(32 * kFinSlices)
@@ -716,15 +675,6 @@ extern "C" int b200seg_accum_f32(float* dst, const float* src, int64_t n, void* 
   CHECK_LAUNCH();
 }
 
-extern "C" int b200seg_bn_eval_params(int32_t c, const float* gamma, const float* beta, float eps,
-                                      const float* running_mean, const float* running_var, float* scale, float* shift,
-                                      void* stream) {
-  if (!gamma || !beta || !running_mean || !running_var || !scale || !shift) return B200SEG_E_BADARG;
-  launch_k(bn_eval_params_kernel, dim3((c + 127) / 128), dim3(128), 0, (cudaStream_t)stream, c, gamma, beta, eps,
-           running_mean, running_var, scale, shift);
-  CHECK_LAUNCH();
-}
-
 extern "C" int b200seg_bn_apply(const void* y, int32_t y_ld, const float* scale, const float* shift, const void* res,
                                 int32_t res_ld, const float* post_scale, int32_t relu, void* z, int32_t z_ld,
                                 int64_t npix, int32_t hw, int32_t c, void* stream) {
@@ -776,8 +726,8 @@ extern "C" int32_t b200seg_bn_bwd_grid(int64_t npix, int32_t c) {
 static int bn_bwd_reduce_launch(const void* dz, int32_t dz_ld, const void* mask, int32_t mask_ld,
                                 const float* post_scale, const void* y, int32_t y_ld, const float* mean,
                                 const float* invstd, int64_t npix, int32_t hw, int32_t c, float* partials,
-                                const BnBwdFold& fold, void* stream) {
-  if (!dz || !y || !mean || !invstd || (!partials && !fold.accum) || c % 8 || c > 2048) return B200SEG_E_BADARG;
+                                double* cells, void* stream) {
+  if (!dz || !y || !mean || !invstd || (!partials && !cells) || c % 8 || c > 2048) return B200SEG_E_BADARG;
   int rows, threads;
   reduce_shape(c, &rows, &threads);
   if (threads > 256) return B200SEG_E_BADARG;
@@ -785,7 +735,7 @@ static int bn_bwd_reduce_launch(const void* dz, int32_t dz_ld, const void* mask,
   const size_t smem = (size_t)rows * (c / 8) * 16 * sizeof(float);
   launch_k(bn_bwd_reduce_kernel, dim3(grid), dim3(threads), smem, (cudaStream_t)stream, (const __nv_bfloat16*)dz,
            dz_ld, (const __nv_bfloat16*)mask, mask_ld, post_scale, (const __nv_bfloat16*)y, y_ld, mean, invstd, npix,
-           hw, c, rows, partials, fold);
+           hw, c, rows, partials, cells);
   CHECK_LAUNCH();
 }
 
@@ -793,23 +743,8 @@ extern "C" int b200seg_bn_bwd_reduce(const void* dz, int32_t dz_ld, const void* 
                                      const float* post_scale, const void* y, int32_t y_ld, const float* mean,
                                      const float* invstd, int64_t npix, int32_t hw, int32_t c, float* partials,
                                      void* stream) {
-  BnBwdFold fold;
-  memset(&fold, 0, sizeof(fold));
-  return bn_bwd_reduce_launch(dz, dz_ld, mask, mask_ld, post_scale, y, y_ld, mean, invstd, npix, hw, c, partials, fold,
-                              stream);
-}
-
-extern "C" int b200seg_bn_bwd_reduce_finalize(const void* dz, int32_t dz_ld, const void* mask, int32_t mask_ld,
-                                              const float* post_scale, const void* y, int32_t y_ld, const float* mean,
-                                              const float* invstd, int64_t npix, int32_t hw, int32_t c, double* accum,
-                                              uint32_t* counter, float* dgamma, float* dbeta, float* c1, float* c2,
-                                              void* stream) {
-  if (!accum || !counter || !c1 || !c2 || (reinterpret_cast<uintptr_t>(accum) & 7)) return B200SEG_E_BADARG;
-  BnBwdFold fold;
-  fold.accum = accum; fold.counter = counter; fold.dgamma = dgamma; fold.dbeta = dbeta; fold.c1 = c1; fold.c2 = c2;
-  fold.count = (float)npix;
-  return bn_bwd_reduce_launch(dz, dz_ld, mask, mask_ld, post_scale, y, y_ld, mean, invstd, npix, hw, c, nullptr, fold,
-                              stream);
+  return bn_bwd_reduce_launch(dz, dz_ld, mask, mask_ld, post_scale, y, y_ld, mean, invstd, npix, hw, c, partials,
+                              nullptr, stream);
 }
 
 extern "C" int b200seg_bn_bwd_finalize(const float* partials, int32_t grid, int32_t c, float count, float* dgamma,
@@ -850,12 +785,8 @@ extern "C" int b200seg_bn_bwd_cells(const void* dz, int32_t dz_ld, const void* m
                                     int64_t npix, int32_t hw, int32_t c, void* stream) {
   if (!dz || !y || !dy || !mean || !invstd || !cells || c % 8 || (reinterpret_cast<uintptr_t>(cells) & 7))
     return B200SEG_E_BADARG;
-  BnBwdFold fold;
-  memset(&fold, 0, sizeof(fold));
-  fold.accum = cells;                 // counter == nullptr: cells only
-  fold.count = (float)npix;
   if (int rc = bn_bwd_reduce_launch(dz, dz_ld, mask, mask_ld, post_scale, y, y_ld, mean, invstd, npix, hw, c, nullptr,
-                                    fold, stream))
+                                    cells, stream))
     return rc;
   launch_k(bn_bwd_apply_kernel, dim3(ew_grid(npix * (c / 8))), dim3(256), 5 * c * sizeof(float), (cudaStream_t)stream,
            (const __nv_bfloat16*)dz, dz_ld, (const __nv_bfloat16*)mask, mask_ld, post_scale, (const __nv_bfloat16*)y,

@@ -71,8 +71,8 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   uint64_t* a_empty = bars + kMaxASlots;
   uint64_t* b_full = bars + 2 * kMaxASlots;        // [kMaxBSlots2] (resident: only [0])
   uint64_t* b_empty = b_full + kMaxBSlots2;
-  uint32_t* ticket = reinterpret_cast<uint32_t*>(b_empty + kMaxBSlots2);
-  float* s_stats = reinterpret_cast<float*>(ticket + 4);   // [kStatSlots][2][cout_pad]
+  // 16 bytes of padding (part of halo_smem_layout's byte count, which sets the ring depths), then the statistics
+  float* s_stats = reinterpret_cast<float*>(b_empty + kMaxBSlots2) + 4;   // [kStatSlots][2][cout_pad]
 
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 8 && lane == 0) {
@@ -235,7 +235,7 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   __syncthreads();
   if (p.emit_stats) {
     if (fold.accum != nullptr) {
-      bn_fold_tail(fold, s_stats, p.cout_pad, ticket);          // statistics finalised by the last CTA of this launch
+      bn_fold_tail(fold, s_stats, p.cout_pad);
     } else {
       float* out = stats_partials + (size_t)blockIdx.x * 2 * p.cout_pad;
       for (int i = threadIdx.x; i < 2 * p.cout_pad; i += kHThreads) {
@@ -252,20 +252,17 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 // Two CTAs may share an SM when their Cout tile needs at most 128 accumulator columns (64 registers per consumer thread)
 // and half of the shared memory: CTAs of DIFFERENT launches (the 0.5x and 1.0x
 // passes, the HRNet branch streams, a PDL successor's prologue) then overlap their fill/drain latencies on one SM, and a
-// 256-tile layer runs as one round of 264 slots instead of two rounds of 132. B200SEG_CORESIDENT=0 restores one CTA/SM.
-static bool halo_coresident_enabled() {
-  static const bool on = []() { const char* e = getenv("B200SEG_CORESIDENT"); return !(e && e[0] == '0'); }();
-  return on;
-}
+// 256-tile layer runs as one round of 264 slots instead of two rounds of 132.
 constexpr size_t kHalfSmBudget = 115712;   // (228 KB - 2 x 1 KB reserved) / 2
 
 // Shared-memory layout of a CTA for a given Cout tile: returns the CTAs per SM it allows (2, 1, or 0 = does not fit).
 struct HaloSmem { int resident, a_slots, b_slots; size_t bytes; };
 static int halo_smem_layout(int BN, int n_tiles, int cchunks, int cout_pad, HaloSmem& L) {
   const size_t b_tile = (size_t)(BN * 128 + 1023) / 1024 * 1024;
-  const size_t fixed = 1024 + (2 * kMaxASlots + 2 * kMaxBSlots2) * 8 + 16 + (size_t)kStatSlots * 2 * cout_pad * 4;
+  const size_t fixed =
+      1024 + (2 * kMaxASlots + 2 * kMaxBSlots2) * 8 + 16 /*padding*/ + (size_t)kStatSlots * 2 * cout_pad * 4;
   const size_t resident_bytes = (size_t)9 * cchunks * b_tile;
-  for (int occ = (halo_coresident_enabled() && BN <= 128) ? 2 : 1; occ >= 1; --occ) {
+  for (int occ = BN <= 128 ? 2 : 1; occ >= 1; --occ) {
     const size_t budget = (occ == 2 ? kHalfSmBudget : (size_t)227 * 1024) - fixed - (size_t)smem_reserve() / occ;
     if (n_tiles == 1 && resident_bytes + 2 * (size_t)kASlotBytes <= budget) {
       const int as_ = (int)((budget - resident_bytes) / kASlotBytes);

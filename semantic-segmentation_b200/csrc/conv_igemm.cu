@@ -55,14 +55,14 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                   float* __restrict__ stats_partials, const __nv_bfloat16* __restrict__ addend, const BnFoldDev fold) {
   static_assert(NB16 >= 1 && NB16 <= (OCC == 2 ? 8 : 16), "accumulator columns exceed the register budget");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [stages][A|B] (1024-aligned) | barriers | ticket | stats[kStatSlots][2][cout_pad]
+  // carve: [stages][A|B] (1024-aligned) | barriers | 16 bytes of padding | stats[kStatSlots][2][cout_pad]
+  // (the padding is part of plan_geom's byte count, which sets the ring depth)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* stage_base = smem;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)p.nstages * p.stage_bytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kMaxStages;
-  uint32_t* ticket = reinterpret_cast<uint32_t*>(bars + 2 * kMaxStages);
-  float* s_stats = reinterpret_cast<float*>(ticket + 4);
+  float* s_stats = reinterpret_cast<float*>(bars + 2 * kMaxStages) + 4;
 
   const uint32_t warp = threadIdx.x >> 5;
   const uint32_t lane = threadIdx.x & 31;
@@ -180,7 +180,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   __syncthreads();
   if (p.emit_stats) {
     if (fold.accum != nullptr) {
-      bn_fold_tail(fold, s_stats, p.cout_pad, ticket);          // statistics finalised by the last CTA of this launch
+      bn_fold_tail(fold, s_stats, p.cout_pad);
     } else {
       float* out = stats_partials + (size_t)blockIdx.x * 2 * p.cout_pad;
       for (int i = threadIdx.x; i < 2 * p.cout_pad; i += kThreads) {
@@ -201,11 +201,6 @@ struct LaunchGeom {
   int ntaps, tap_dh[9], tap_dw[9], tap_w[9], wtaps;   // wtaps = taps dimension of the weight tensor
   int out_fp32, has_bias, emit_stats, force_kc;
 };
-
-static bool coresident_enabled() {
-  static const bool on = []() { const char* e = getenv("B200SEG_CORESIDENT"); return !(e && e[0] == '0'); }();
-  return on;
-}
 
 static int plan_geom(const LaunchGeom& g, ConvPlan* pl) {
   if (g.n <= 0 || g.sub_h <= 0 || g.sub_w <= 0) return B200SEG_E_BADARG;
@@ -256,11 +251,11 @@ static int plan_geom(const LaunchGeom& g, ConvPlan* pl) {
   pl->b_bytes = pl->BN * KC * 2;
   pl->stage_bytes = (pl->a_bytes + pl->b_bytes + 1023) / 1024 * 1024;
   pl->acc_regs = pl->BN / 2;
-  size_t fixed = 1024 /*align slack*/ + 2 * kMaxStages * 8 + 16 + (size_t)kStatSlots * 2 * pl->cout_pad * 4;
+  size_t fixed = 1024 /*align slack*/ + 2 * kMaxStages * 8 + 16 /*padding*/ + (size_t)kStatSlots * 2 * pl->cout_pad * 4;
   // two CTAs per SM for narrow Cout tiles (<= 128 accumulator columns = 64 registers per consumer thread, half of the
   // shared memory each), so that CTAs of different launches overlap their fill / drain latencies on one SM; else one CTA
   // with the deepest ring
-  int occ = (coresident_enabled() && pl->BN <= 128) ? 2 : 1;
+  int occ = pl->BN <= 128 ? 2 : 1;
   int nst = 0;
   for (; occ >= 1; --occ) {
     const size_t budget = (occ == 2 ? kHalfSmBudget : (size_t)227 * 1024) - fixed - (size_t)smem_reserve() / occ;
@@ -351,12 +346,7 @@ int make_bn_fold(const b200seg_bn_fold* f, int cout, BnFoldDev* out) {
   memset(&d, 0, sizeof(d));
   if (f) {
     if (!f->accum || f->c != cout || (reinterpret_cast<uintptr_t>(f->accum) & 7)) return B200SEG_E_BADARG;
-    // counter == NULL: deferred mode, only the cells are touched (see bn_fold.cuh)
-    if (f->counter && (!f->scale || !f->shift || !f->mean || !f->invstd || f->count <= 0.f)) return B200SEG_E_BADARG;
-    d.accum = f->accum; d.counter = f->counter; d.gamma = f->gamma; d.beta = f->beta;
-    d.scale = f->scale; d.shift = f->shift; d.mean = f->mean; d.invstd = f->invstd; d.batch_out = f->batch_stats_out;
-    d.running_mean = f->running_mean; d.running_var = f->running_var; d.nbt = (long long*)f->num_batches_tracked;
-    d.eps = f->eps; d.momentum = f->momentum; d.count = f->count; d.C = f->c;
+    d.accum = f->accum;   // only the cells are touched (see bn_fold.cuh)
   }
   *out = d;
   return 0;
@@ -566,7 +556,6 @@ extern "C" int b200seg_conv2d_fwd_affine(const b200seg_conv_desc* d, const void*
   fd.scale = const_cast<float*>(scale);
   fd.shift = const_cast<float*>(shift);
   fd.relu = relu ? 1 : 0;
-  fd.C = d->cout;
   if (d->ksize == 3 && d->stride == 1 && d->cout % 16 == 0 && d->reserved == 0 && conv_dil(d) == 1)
     return conv3x3_halo_launch(d->n, d->h, d->w, d->cin, d->x_ld, x, d->cout, w_ohwi, nullptr, y, d->y_ld, nullptr,
                                nullptr, addend, addend_ld, 0, (cudaStream_t)stream, nullptr, &fd);

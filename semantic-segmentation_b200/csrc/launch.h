@@ -1,22 +1,13 @@
 // Kernel launch helper: every launch carries the programmatic-stream-serialization attribute (PDL) so the next kernel's
 // prologue overlaps this kernel's body (see ptx.cuh pdl_*). Works under stream capture (the edge becomes a programmatic
-// graph dependency). B200SEG_PDL=0 in the environment falls back to plain serialized launches (A/B measurements).
+// graph dependency).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdlib>
 
 namespace b200seg {
 
-inline bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B200SEG_PDL");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v != 0;
-}
-
-// B200SEG_DRY (measurement only, tools/gpu_r2_call10.sh): every launch of the library becomes an empty kernel that keeps
+// B200SEG_DRY (measurement only): every launch of the library becomes an empty kernel that keeps
 // the stream / programmatic dependency structure: 1 = one warp, 2 = the real grid and block dimensions (no shared
 // memory). A captured step then replays at the launch-and-dependency floor of its program; results are garbage.
 inline int dry_mode() {
@@ -41,7 +32,7 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = 1;
   if (const int dry = dry_mode()) {
     if (dry == 1) { cfg.gridDim = dim3(1); cfg.blockDim = dim3(32); }
     cfg.dynamicSmemBytes = 0;

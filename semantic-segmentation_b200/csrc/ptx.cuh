@@ -78,18 +78,13 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t phase) { mbar_
 // Because *every* kernel executes pdl_wait before it completes, completion is transitive along the stream.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-// Late trigger (default; -DB200SEG_PDL_EARLY builds the variant that triggers at the start of every kernel): a dependent grid that becomes resident at the START
-// of its predecessor holds registers and shared memory on the SMs for the predecessor's whole duration while it
-// sits in griddepcontrol.wait - on a step bound by what fits on the SMs that residency is paid by the other streams. The
-// default therefore triggers the dependent when a CTA has finished its main loop (pdl_launch_late), so only the successor's
-// prologue overlaps the predecessor's tail; kernels without an explicit late trigger fall back to the implicit one at exit.
-#ifndef B200SEG_PDL_EARLY
+// Late trigger: a dependent grid that becomes resident at the START of its predecessor holds registers and shared memory
+// on the SMs for the predecessor's whole duration while it sits in griddepcontrol.wait - on a step bound by what fits on
+// the SMs that residency is paid by the other streams. Kernels therefore trigger the dependent when a CTA has finished its
+// main loop (pdl_launch_late), so only the successor's prologue overlaps the predecessor's tail; kernels without an
+// explicit late trigger fall back to the implicit one at exit.
 __device__ __forceinline__ void pdl_sync() { pdl_wait(); }
 __device__ __forceinline__ void pdl_launch_late() { pdl_launch(); }
-#else
-__device__ __forceinline__ void pdl_sync() { pdl_wait(); pdl_launch(); }
-__device__ __forceinline__ void pdl_launch_late() {}
-#endif
 
 // ---------------------------------------------------------------- TMA
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {

@@ -34,6 +34,26 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(T, s) and not hasattr(L, s), s
 
 
+def test_library_reads_only_the_known_environment_switches():
+    """The Python and the C++ code name every environment variable they read as a "B200SEG_..." string literal. The set
+    is fixed, so an execution variant selected by the environment cannot come back without this list changing; the only
+    compile-time B200SEG_ switch is the mbarrier spin bound."""
+    pkg = os.path.join(ROOT, "semantic-segmentation_b200")
+    names, guarded = set(), set()
+    for dp, _, files in os.walk(pkg):
+        for f in files:
+            if f.endswith((".py", ".cu", ".cuh", ".h")):
+                txt = open(os.path.join(dp, f)).read()
+                names |= set(re.findall(r'"(B200SEG_[A-Z0-9_]+)"', txt))
+                if os.path.basename(dp) == "csrc":
+                    guarded |= set(re.findall(r"^[ \t]*#[ \t]*if(?:n?def)?\b.*?\b(B200SEG_\w+)", txt, flags=re.M))
+    tune = {"B200SEG_" + k for k in ("CONV_MIN_CLK", "WGRAD_MIN_CLK", "EW_ITEMS", "EW_CTAS_PER_SM", "RED_ITEMS",
+                                     "RED_CTAS_PER_SM", "RS_ITEMS")}
+    assert names == {"B200SEG_LIB_VARIANT", "B200SEG_OVERLAY", "B200SEG_HRNET_CHECKPOINT", "B200SEG_DRY"} | tune, \
+        sorted(names)
+    assert guarded == {"B200SEG_SPIN_LIMIT"}, sorted(guarded)
+
+
 def test_no_torch_types_in_the_abi():
     src = open(os.path.join(ROOT, "include", "b200seg.h")).read()
     assert "torch" not in src.lower() and "at::" not in src and "#include <cuda" not in src

@@ -17,7 +17,7 @@ group breaks these.
 The widest Cout tiles still keep a few bytes of spill next to their 128 (OCC 1) or 64 (OCC 2) accumulator registers,
 all of it outside the MMA region except in halo <2, 8> (ptxas -v, stack / spill stores / spill loads in bytes):
 halo <1, 16> 8 / 12 / 16, halo <2, 7> 16 / 16 / 68, halo <2, 8> 48 / 88 / 176, igemm <1, 16> 16 / 20 / 20,
-igemm <2, 7> 8 / 16 / 16, igemm <2, 8> 64 / 288 / 420. halo <2, 8> is never launched: at BN 128 only three weight-ring
+igemm <2, 7> 8 / 16 / 16, igemm <2, 8> 64 / 288 / 412. halo <2, 8> is never launched: at BN 128 only three weight-ring
 slots fit in half an SM, and halo_smem_layout asks for four before it picks two CTAs per SM. SPILLING lists these
 six, and the test fails when one of them stops spilling so that the list stays exact."""
 import os

@@ -3,8 +3,7 @@
   * default data-parallel mode (BatchNorm statistics local to each GPU, ONE NCCL all-reduce over the flat gradient
     buffer): every rank must end up with the mean of the per-rank gradients;
   * SyncBN mode (opt-in, `syncbn=True`): statistics exchanged through NVLink peer memory inside the BN finalisers must
-    reproduce the single-GPU step on the concatenated batch. That test passed on 2 GPUs at commit 05390e9; later
-    multi-stream changes were not re-validated, so it only runs with B200SEG_TEST_SYNCBN=1."""
+    reproduce the single-GPU step on the concatenated batch, eager and graph-captured."""
 import os
 
 import pytest

@@ -31,12 +31,7 @@ def test_two_scale_step_flops_and_launch_structure():
     assert wgrad[0] == fwd[0] - 3 and dgrad[0] == fwd[0] - 3 - 2
     assert abs(fwd[1] - 1.25 * 3.0546) <= 0.02                           # 1.25 x one full-resolution _fwd
     assert r["bn_finalize"][0] == 2 * 316 and r["bn_bwd_finalize"][0] == r["bn_bwd_reduce"][0] == r["bn_bwd_apply"][0]
-    # opt-in program (B200SEG_FUSED_BN=1): statistics finalised inside the producing launches
-    f = _trace("--arch", "ocrnet.HRNet_Mscale", "--fused-bn")
-    assert f["conv2d_fwd_bn"][0] == 2 * 316 and "bn_finalize" not in f and "bn_bwd_finalize" not in f
-    assert f["conv2d_fwd_bn"][0] + f["conv2d_fwd"][0] == 2 * 322
-    assert r["total"][0] - f["total"][0] == 2 * 316 + r["bn_bwd_finalize"][0]     # launches the fused finalisers save
-    # default training program with per-GPU statistics (B200SEG_BN_CELLS=1): deferred finalisation - a bn_finalize launch
+    # default training program with per-GPU statistics: deferred finalisation - a bn_finalize launch
     # remains only in front of the fuse layers (their consumers read scale / shift), no bn_bwd_finalize at all
     c = _trace("--arch", "ocrnet.HRNet_Mscale", "--bn-cells")
     assert c["bn_apply_cells"][0] + c["bn_finalize"][0] == 2 * 316 and "bn_bwd_finalize" not in c

@@ -40,8 +40,8 @@ def _key(name, args, sizes):
         opt = (args[2], args[4] is not None, args[5], args[7])
     elif name == "b200seg_conv2d_fwd_add":    # (d, x, w, bias, addend, addend_ld, y, stats, grid, stream)
         opt = (args[5], args[7] is not None)
-    elif name == "b200seg_conv2d_fwd_bn":     # (d, x, w, bias, y, fold, stream): counter NULL = deferred cells
-        opt = (args[5]._obj.counter is not None,)
+    elif name == "b200seg_conv2d_fwd_bn":     # (d, x, w, bias, y, fold, stream)
+        opt = ()
     elif name == "b200seg_conv2d_fwd_affine":  # (d, x, w, scale, shift, relu, addend, addend_ld, y, stream)
         opt = (args[5], args[6] is not None, args[7])
     else:                                     # (d, x, w, bias, y, stats, grid, stream)
@@ -99,19 +99,12 @@ def make_launch(L, name, d, opt, torch):
         add = rnd(d.n, ho, wo, add_ld) if has_add else None
         return (lambda: check(L.b200seg_conv2d_fwd_affine(ctypes.byref(d), ptr(x), ptr(w), ptr(scale), ptr(shift), relu,
                                                           ptr(add), add_ld, ptr(y), stream_ptr()))), keep + (add,)
-    # fwd_bn: statistics into self-clearing fp64 cells (counter set: finalised by the last CTA, as in the step)
-    c16 = (d.cout + 15) // 16 * 16
-    cells = torch.zeros(2 * c16, dtype=torch.float64, device=dev)
-    par = torch.empty((4, d.cout), device=dev)
-    gamma, beta = torch.ones(d.cout, device=dev), torch.zeros(d.cout, device=dev)
-    counter = torch.zeros(1, dtype=torch.int32, device=dev) if opt[0] else None
+    # fwd_bn: statistics added to the layer's fp64 cells (deferred finalisation, as in the step)
+    cells = torch.zeros(2 * ((d.cout + 15) // 16 * 16), dtype=torch.float64, device=dev)
     f = _lib.BnFold()
-    f.accum, f.counter = ptr(cells), ptr(counter)
-    f.gamma, f.beta = ptr(gamma), ptr(beta)
-    f.scale, f.shift, f.mean, f.invstd = ptr(par[0]), ptr(par[1]), ptr(par[2]), ptr(par[3])
-    f.eps, f.momentum, f.count, f.c = 1e-5, 0.1, float(d.n * ho * wo), d.cout
+    f.accum, f.c = ptr(cells), d.cout
     return (lambda: check(L.b200seg_conv2d_fwd_bn(ctypes.byref(d), ptr(x), ptr(w), ptr(bias), ptr(y), ctypes.byref(f),
-                                                  stream_ptr()))), keep + (cells, par, gamma, beta, counter, f)
+                                                  stream_ptr()))), keep + (cells, f)
 
 
 def main():

@@ -1,7 +1,6 @@
 #!/usr/bin/env python
 """cfg5 timing (GPU): ocrnet.HRNet_Mscale three-scale inference {0.5, 1.0, 2.0} of one 1024x2048 frame + device-side
-argmax / confusion matrix, eager and CUDA-graph replay. B200SEG_EVAL_FUSED=0/1 switches the fused conv+BN(+res)+ReLU
-epilogue. Prints one JSON line."""
+argmax / confusion matrix, eager and CUDA-graph replay. Prints one JSON line."""
 import json
 import os
 import sys
@@ -35,7 +34,6 @@ def main():
         pred = net({"images": images})["pred"]
         out["pred_checksum"] = float(pred.float().abs().mean())
         out["argmax_hist"] = torch.bincount(pred.argmax(1).flatten(), minlength=19)[:6].tolist()
-    out["fused"] = os.environ.get("B200SEG_EVAL_FUSED", "1")
     print(json.dumps(out))
 
 

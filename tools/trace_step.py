@@ -84,13 +84,10 @@ def main():
                     help="sustained dense bf16 TFLOP/s (MEASURED_PEAKS.json)")
     ap.add_argument("--gbs", type=float, default=pk["hbm_gbs"], help="HBM copy bandwidth GB/s (MEASURED_PEAKS.json)")
     ap.add_argument("--top", type=int, default=0, help="also list the N largest launches by roofline time")
-    ap.add_argument("--fused-bn", action="store_true",
-                    help="trace the opt-in program with the BatchNorm finalisation inside the producing launches "
-                         "(B200SEG_FUSED_BN=1) instead of the default bn_finalize / bn_bwd_finalize launches")
     ap.add_argument("--bn-cells", action="store_true",
-                    help="trace the training default with per-GPU statistics (B200SEG_BN_CELLS=1): deferred BatchNorm "
-                         "finalisation inside the consuming apply passes; without the flag: the program with separate "
-                         "bn_finalize / bn_bwd_finalize launches (SyncBN, B200SEG_BN_CELLS=0)")
+                    help="trace the training default with per-GPU statistics: deferred BatchNorm finalisation inside "
+                         "the consuming apply passes; without the flag: the program with separate bn_finalize / "
+                         "bn_bwd_finalize launches (SyncBN)")
     args = ap.parse_args()
     if __debug__:
         sys.exit("run with python -O (the wrappers assert is_cuda)")
@@ -122,17 +119,12 @@ def main():
         mask = torch.empty((sum(c for _b, c, _p in A.wrn_drop_layout(net.hcfg)),), dtype=torch.float32, device=dev)
     else:
         mask = torch.empty((1, net.ocfg["mid_channels"]), dtype=torch.float32, device=dev)
-    bnfold = None
-    if args.fused_bn:
-        bnfold = {n[: -len(".running_mean")]: (torch.empty(2 * ((v.shape[0] + 15) // 16 * 16), dtype=torch.float64, device=dev),
-                                               torch.empty(1, dtype=torch.int32, device=dev))
-                  for n, v in tensors.items() if n.endswith(".running_mean")}
     bncells = None
     if args.bn_cells:
         bncells = {n[: -len(".running_mean")]: (torch.empty(2 * ((v.shape[0] + 15) // 16 * 16), dtype=torch.float64, device=dev),
                                                 torch.empty(2 * v.shape[0], dtype=torch.float64, device=dev))
                    for n, v in tensors.items() if n.endswith(".running_mean")}
-    E = EN.Engine(tensors, grads, packed, True, mask, bnfold=bnfold, bncells=bncells)
+    E = EN.Engine(tensors, grads, packed, True, mask, bncells=bncells)
     M.train_loss(E, images, gts, args.arch, net.hcfg, net.ocfg)
     n_fwd = len(EVENTS)
     M.run_backward(E)
