@@ -7,7 +7,8 @@
 // ([channel group][18][10][8 channels], 16 bytes per pixel of a plane, one TMA box of 8 channels per plane), so every
 // 8-pixel run of a plane is one 8 x 16-byte core matrix at any pixel offset:
 //     start = plane + (kh*10 + kw) * 16 B,   SBO = 10 * 16 B (next tile row),   LBO = plane pitch (next channel group)
-// The weights use the same no-swizzle layout ([channel group][BN][8 channels]).
+// The weights use the same no-swizzle layout ([channel group][BN][8 channels]). The last chunk of a Cin that is not a
+// multiple of 64 fetches only the planes its K steps read (both operands), not planes that lie wholly past Cin.
 //
 // Roles (288 threads): warps 0-7 = two consumer warpgroups (tile rows 0-7 / 8-15: MMA + epilogue), warp 8 = TMA producer.
 // Weights: resident in shared memory for the whole persistent CTA when they fit (C <= 96: the HBM-bound layers), else
@@ -85,14 +86,17 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   if (p.emit_stats)
     for (int i = threadIdx.x; i < kStatSlots * 2 * p.cout_pad; i += kHThreads) s_stats[i] = 0.f;
   __syncthreads();
+  // Channel-group planes fetched per chunk: the MMAs of a chunk with KS K steps read planes 0 .. 2 KS - 1 only, so the last
+  // chunk of a Cin that is not a multiple of 64 skips the planes that would lie wholly past Cin (48: 2 of 8, 96: 4, 720: 6).
+  const int planes_last = 2 * p.ksteps_last;
   // Resident weights are static for the whole step (written by the pack kernels, which never trigger a programmatic
   // launch): fetch them while the previous kernel on the stream is still draining.
   if (warp == 8 && p.resident) {
     if (elect_one()) {
-      mbar_arrive_expect_tx(&b_full[0], 9 * p.cchunks * p.b_tile_bytes);
+      mbar_arrive_expect_tx(&b_full[0], 9 * ((p.cchunks - 1) * 8 + planes_last) * p.BN * 16);
       for (int cc = 0; cc < p.cchunks; ++cc)
         for (int t = 0; t < 9; ++t)
-          for (int j = 0; j < 8; ++j)
+          for (int j = 0; j < (cc == p.cchunks - 1 ? planes_last : 8); ++j)
             tma_load_3d(&tmB, &b_full[0], b_base + (size_t)(cc * 9 + t) * p.b_tile_bytes + j * p.BN * 16, cc * 64 + 8 * j,
                         t, 0);
     }
@@ -111,17 +115,18 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         const int th_i = (m_tile / p.tiles_w) % p.tiles_h;
         const int img = m_tile / (p.tiles_w * p.tiles_h);
         for (int cc = 0; cc < p.cchunks; ++cc) {
+          const int planes = cc == p.cchunks - 1 ? planes_last : 8;
           mbar_wait(&a_empty[a_slot], a_phase ^ 1);
-          mbar_arrive_expect_tx(&a_full[a_slot], 8 * kPlaneBytes);
-          for (int j = 0; j < 8; ++j)
+          mbar_arrive_expect_tx(&a_full[a_slot], planes * kPlaneBytes);
+          for (int j = 0; j < planes; ++j)
             tma_load_4d(&tmA, &a_full[a_slot], a_base + (size_t)a_slot * kASlotBytes + j * kPlane, cc * 64 + 8 * j,
                         tw_i * kTW - 1, th_i * kTH - 1, img);
           if (++a_slot == p.a_slots) { a_slot = 0; a_phase ^= 1; }
           if (!p.resident) {
             for (int t = 0; t < 9; ++t) {
               mbar_wait(&b_empty[b_slot], b_phase ^ 1);
-              mbar_arrive_expect_tx(&b_full[b_slot], p.b_tile_bytes);
-              for (int j = 0; j < 8; ++j)
+              mbar_arrive_expect_tx(&b_full[b_slot], planes * p.BN * 16);
+              for (int j = 0; j < planes; ++j)
                 tma_load_3d(&tmB, &b_full[b_slot], b_base + (size_t)b_slot * p.b_tile_bytes + j * p.BN * 16,
                             cc * 64 + 8 * j, t, n_tile * p.BN);
               if (++b_slot == p.b_slots) { b_slot = 0; b_phase ^= 1; }
