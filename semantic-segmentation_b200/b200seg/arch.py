@@ -18,13 +18,19 @@ HRNET_W48 = dict(
 # config.py:157-159 (OCR), :130 (SEGATTN_BOT_CH), network/ocrnet.py:63 (dropout)
 OCR_DEFAULT = dict(mid_channels=512, key_channels=256, num_classes=19, segattn_bot_ch=256, dropout=0.05)
 
-ARCHS = ("ocrnet.HRNet_Mscale", "ocrnet.HRNet", "basic.HRNet", "mscale.HRNet", "deepv3.DeepV3PlusW38")
+ARCHS = ("ocrnet.HRNet_Mscale", "ocrnet.HRNet", "basic.HRNet", "mscale.HRNet", "deepv3.DeepV3PlusW38",
+         "mscale.DeepV3W38")
 
 
 def is_two_scale(arch):
     """Architectures whose training forward is the hierarchical two-scale pass (MscaleOCR.two_scale_forward,
     network/ocrnet.py:264-334; MscaleBase.two_scale_forward, network/mscale.py:182-231)."""
-    return arch in ("ocrnet.HRNet_Mscale", "mscale.HRNet")
+    return arch in ("ocrnet.HRNet_Mscale", "mscale.HRNet", "mscale.DeepV3W38")
+
+
+def has_wrn38_trunk(arch):
+    """Architectures built on the WideResNet-38 trunk, ASPP and 304-channel decoder (DeepV3Plus, MscaleV3Plus)."""
+    return arch in ("deepv3.DeepV3PlusW38", "mscale.DeepV3W38")
 
 
 def has_ocr(arch):
@@ -58,9 +64,11 @@ def wrn_drop_layout(wcfg=WRN38):
             if drop is not None and len(ch) == 3]
 
 
-def deepv3_tensor_specs(num_classes=19, wcfg=WRN38):
+def deepv3_tensor_specs(num_classes=19, wcfg=WRN38, bot_ch=256, scale_attn=False):
     """(name, shape, kind) of deepv3.DeepV3PlusW38 in the reference's registration order (network/deepv3.py:46-65,
-    network/utils.py:171-202)."""
+    network/utils.py:171-202). scale_attn: mscale.DeepV3W38 (MscaleV3Plus.__init__, network/mscale.py:236-277), whose
+    decoder `final` is bot_ch (cfg.MODEL.SEGATTN_BOT_CH) wide and is followed by the attention head on the same
+    304-channel concat."""
     out = []
 
     def conv(name, o, i, k):
@@ -93,9 +101,13 @@ def deepv3_tensor_specs(num_classes=19, wcfg=WRN38):
     conv("aspp.img_conv.0", 256, high, 1); bn("aspp.img_conv.1", 256)
     conv("bot_fine", 48, s2_ch, 1)
     conv("bot_aspp", 256, 256 * (2 + len(ASPP_RATES)), 1)
-    conv("final.0", 256, 256 + 48, 3); bn("final.1", 256)
-    conv("final.3", 256, 256, 3); bn("final.4", 256)
-    conv("final.6", num_classes, 256, 1)
+    conv("final.0", bot_ch, 256 + 48, 3); bn("final.1", bot_ch)
+    conv("final.3", bot_ch, bot_ch, 3); bn("final.4", bot_ch)
+    conv("final.6", num_classes, bot_ch, 1)
+    if scale_attn:      # make_attn_head(304, 1) (network/utils.py:343-367)
+        conv("scale_attn.conv0", bot_ch, 256 + 48, 3); bn("scale_attn.bn0", bot_ch)
+        conv("scale_attn.conv1", bot_ch, bot_ch, 3); bn("scale_attn.bn1", bot_ch)
+        conv("scale_attn.conv2", 1, bot_ch, 1)
     return out
 
 
@@ -117,6 +129,9 @@ def tensor_specs(arch, hcfg=HRNET_W48, ocfg=OCR_DEFAULT):
     """-> list of (name, shape, kind) with kind in {'conv_w','conv_b','bn_w','bn_b','bn_rm','bn_rv','bn_nbt'}."""
     if arch == "deepv3.DeepV3PlusW38":
         return deepv3_tensor_specs(ocfg["num_classes"], hcfg if "structure" in hcfg else WRN38)
+    if arch == "mscale.DeepV3W38":
+        return deepv3_tensor_specs(ocfg["num_classes"], hcfg if "structure" in hcfg else WRN38,
+                                   ocfg["segattn_bot_ch"], scale_attn=True)
     out = []
 
     def conv(name, o, i, k, bias=False):

@@ -334,9 +334,15 @@ class Engine:
         if self.training:
             assert x.stats is not None, "pre-activation BN needs the batch statistics of its input"
             n, h, w, _ = x.t.shape
-            par = raw.bn_finalize(x.stats, n * h * w, self.p[bname + ".weight"], self.p[bname + ".bias"], BN_EPS,
-                                  BN_MOMENTUM, self.p[bname + ".running_mean"], self.p[bname + ".running_var"],
-                                  self.p[bname + ".num_batches_tracked"], c, sync=self._sync(bname, 0))
+            if self.bstat is not None:     # concurrent scale passes: running statistics updated once after the join
+                self.bn_seen.add(bname)
+                par = raw.bn_finalize(x.stats, n * h * w, self.p[bname + ".weight"], self.p[bname + ".bias"], BN_EPS,
+                                      BN_MOMENTUM, None, None, None, c, batch_out=self.bstat[bname],
+                                      sync=self._sync(bname, 0))
+            else:
+                par = raw.bn_finalize(x.stats, n * h * w, self.p[bname + ".weight"], self.p[bname + ".bias"], BN_EPS,
+                                      BN_MOMENTUM, self.p[bname + ".running_mean"], self.p[bname + ".running_var"],
+                                      self.p[bname + ".num_batches_tracked"], c, sync=self._sync(bname, 0))
         else:
             par = self.eval_bn[bname]
         a = raw.bn_apply(x.t, par[0], par[1], None, post_scale, True)

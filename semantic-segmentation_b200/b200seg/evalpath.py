@@ -4,6 +4,7 @@ reference's output assembly in fp32 NCHW on the device.
   ocrnet.HRNet_Mscale : MscaleOCR.nscale_forward when cfg.MODEL.N_SCALES is set (network/ocrnet.py:185-262), else the
                         eval branch of two_scale_forward (:264-327)
   mscale.HRNet        : MscaleBase.nscale_forward / two_scale_forward eval branches (network/mscale.py:114-231)
+  mscale.DeepV3W38    : the same assembly over the WRN-38 / ASPP / decoder pass (MscaleV3Plus._fwd, :296-328)
   ocrnet.HRNet        : OCRNet.forward eval branch (:104-122)
   basic.HRNet         : Basic.forward eval branch (network/basic.py:50-64)
   deepv3.DeepV3PlusW38: DeepV3Plus.forward eval branch (network/deepv3.py:73-96)
@@ -44,8 +45,8 @@ def eval_forward(module, images):
     # ONE launch each (raw.conv2d_fwd_affine).
     E.eval_bn = module._eval_bn_params()
     arch = module.arch
-    if arch == "deepv3.DeepV3PlusW38":          # DeepV3Plus.forward eval branch (network/deepv3.py:73-96)
-        head = M.deepv3_pass(E, images, module.hcfg)
+    if A.has_wrn38_trunk(arch) and not A.is_two_scale(arch):   # DeepV3Plus.forward eval branch (deepv3.py:73-96)
+        head, _ = M.deepv3_pass(E, images, module.hcfg, (H, W), None)
         return {"pred": raw.resize_to_nchw(head.logits, 19, H, W)}
     if not A.is_two_scale(arch):
         return {"pred": _pass(module, E, images, (H, W))["cls_out"]}

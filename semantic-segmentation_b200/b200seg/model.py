@@ -249,19 +249,21 @@ def wrn_block(E, p, x, in_ch, ch, stride, dil, drop_mask):
     return E.conv_sum(t, c + ".conv3", 1, 1, 1, addend=short, want_stats=True)
 
 
-def deepv3_pass(E, images, wcfg):
-    """DeepV3Plus.forward up to the half-resolution logits (network/deepv3.py:75-88): WRN-38 trunk (output stride 8),
-    ASPP (network/utils.py:204-216), decoder. Returns the logit HeadRec [n, H/2, W/2, 19]."""
-    from . import arch as A
-    n, _, H, W = images.shape
-    x16 = Act(raw.image_prep(images, H, W), needs_grad=False)
+def deepv3_pass(E, images, wcfg, size_hw, drop_mask):
+    """DeepV3Plus.forward up to the half-resolution logits (network/deepv3.py:75-88), MscaleV3Plus._fwd up to its two
+    heads (network/mscale.py:296-316): WRN-38 trunk (output stride 8), ASPP (network/utils.py:204-216), decoder.
+    size_hw: pass input size (ResizeX folded into image_prep); drop_mask: fp32 Dropout2d multipliers of mod6 / mod7
+    in A.wrn_drop_layout order, or None. Returns (logit HeadRec [n, h/2, w/2, 19], decoder concat Act
+    [n, h/2, w/2, 304] = [bot_fine(s2) | up(bot_aspp(aspp))])."""
+    n = images.shape[0]
+    x16 = Act(raw.image_prep(images, size_hw[0], size_hw[1]), needs_grad=False)
     x = E.conv_sum(x16, "backbone.mod1.conv1", 3)
     feats = {}
     drop_masks = {}
-    if E.training and E.drop_mask is not None:
+    if drop_mask is not None:
         off = 0
         for bp, c, _p in A.wrn_drop_layout(wcfg):
-            drop_masks[bp] = E.drop_mask[off:off + n * c].view(n, c)
+            drop_masks[bp] = drop_mask[off:off + n * c].view(n, c)
             off += n * c
     for mod, blk, in_ch, ch, stride, dil, drop in A.wrn_block_plan(wcfg):
         if blk == "block1" and mod in ("mod2", "mod3"):
@@ -290,13 +292,18 @@ def deepv3_pass(E, images, wcfg):
     E.slice_marker(cat2, [(conv_s2, 0, 48), (up, 48, 304)])
     t = E.conv_bn(cat2, "final.0", "final.1", 3)
     t = E.conv_bn(t, "final.3", "final.4", 3)
-    return E.conv_head(t, "final.6", bias=False)
+    return E.conv_head(t, "final.6", bias=False), cat2
 
 
 # ----------------------------------------------------------------------------------------------- per-scale pass
-def scale_pass(E, images, size_hw, arch, hcfg, ocfg):
+def scale_pass(E, images, size_hw, arch, hcfg, ocfg, drop_mask=None):
     """MscaleOCR._fwd (network/ocrnet.py:170-183) up to the quarter-resolution maps (the x4 Upsample is fused into the
-    blend/loss kernels). images: fp32 NCHW; size_hw: pass input size (ResizeX folded into image_prep)."""
+    blend/loss kernels). images: fp32 NCHW; size_hw: pass input size (ResizeX folded into image_prep).
+    mscale.DeepV3W38: MscaleV3Plus._fwd (network/mscale.py:296-328) up to the half-resolution maps; drop_mask: this
+    pass' WRN-38 Dropout2d multipliers (deepv3_pass)."""
+    if arch == "mscale.DeepV3W38":     # both heads read the decoder concat
+        cls, cat = deepv3_pass(E, images, hcfg, size_hw, drop_mask)
+        return dict(cls=cls, aux=None, attn=attn_head(E, cat))
     x16 = Act(raw.image_prep(images, size_hw[0], size_hw[1]), needs_grad=False)
     feats = hrnet_forward(E, x16, hcfg)
     if arch == "basic.HRNet":
@@ -311,7 +318,9 @@ def scale_pass(E, images, size_hw, arch, hcfg, ocfg):
 def train_loss(E, images, gts, arch, hcfg, ocfg, lo_scale=0.5, ocr_alpha=0.4, sup_wt=0.0, ignore_index=255, E_lo=None,
                loss_kind="ce", img_wt=(1.0, False), ocr_aux_rmi=False):
     """Training forward + loss. ocrnet.HRNet_Mscale: MscaleOCR.two_scale_forward (network/ocrnet.py:264-319);
-    mscale.HRNet: MscaleBase.two_scale_forward (network/mscale.py:182-220; one head, no auxiliary loss);
+    mscale.HRNet, mscale.DeepV3W38: MscaleBase.two_scale_forward (network/mscale.py:182-220; one head, no auxiliary
+    loss; the DeepLab model's maps are on the half-resolution grid of each pass); deepv3.DeepV3PlusW38:
+    DeepV3Plus.forward (network/deepv3.py:73-96);
     ocrnet.HRNet: OCRNet.forward (:104-122); basic.HRNet: Basic.forward (network/basic.py:50-64).
     Returns the fp32 loss vector [total, cls, aux, sup_lo, sup_hi, rmi, aux rmi, 0]; pushes the loss backward on the
     tape. loss_kind "ce": CrossEntropyLoss2d (loss/utils.py:133-134); "rmi": RMILoss (loss/rmi.py:70-215) = sigmoid BCE
@@ -328,22 +337,28 @@ def train_loss(E, images, gts, arch, hcfg, ocfg, lo_scale=0.5, ocr_alpha=0.4, su
     two_scale = A.is_two_scale(arch)
     lo = None
     main = torch.cuda.current_stream() if images.is_cuda else None
-    deepv3 = arch == "deepv3.DeepV3PlusW38"
     par = two_scale and E_lo is not None and E_lo.stream is not None
     if not par:
         E_lo = E
+    # WRN-38 Dropout2d multipliers: one set per scale pass, [lo | hi] when two-scale (each pass draws its own masks)
+    lo_mask = hi_mask = None
+    if A.has_wrn38_trunk(arch) and E.drop_mask is not None:
+        hi_mask = E.drop_mask
+        if two_scale:
+            half = E.drop_mask.numel() // 2
+            lo_mask, hi_mask = E.drop_mask[:half], E.drop_mask[half:]
     if two_scale:
         hm, wm = int(H * lo_scale), int(W * lo_scale)      # ResizeX: floor(in * scale)
         if par:
             E_lo.stream.wait_stream(main)
             with torch.cuda.stream(E_lo.stream):
-                lo = scale_pass(E_lo, images, (hm, wm), arch, hcfg, ocfg)
+                lo = scale_pass(E_lo, images, (hm, wm), arch, hcfg, ocfg, lo_mask)
         else:
-            lo = scale_pass(E, images, (hm, wm), arch, hcfg, ocfg)
-    if deepv3:
-        hi = dict(cls=deepv3_pass(E, images, hcfg), aux=None, attn=None)
+            lo = scale_pass(E, images, (hm, wm), arch, hcfg, ocfg, lo_mask)
+    if A.has_wrn38_trunk(arch) and not two_scale:
+        hi = dict(cls=deepv3_pass(E, images, hcfg, (H, W), hi_mask)[0], aux=None, attn=None)
     else:
-        hi = scale_pass(E, images, (H, W), arch, hcfg, ocfg)
+        hi = scale_pass(E, images, (H, W), arch, hcfg, ocfg, hi_mask)
     if par:
         main.wait_stream(E_lo.stream)
     nheads = 2 if A.has_ocr(arch) else 1

@@ -107,7 +107,7 @@ class _PublishGrads(torch.autograd.Function):
 class B200SegModule(nn.Module):
     def __init__(self, arch, num_classes=19, criterion=None, hcfg=None, ocfg=None, lo_scale=0.5, ocr_alpha=0.4,
                  supervised_mscale_wt=0.0, ignore_index=255, n_scales=None, use_cuda_graph=True,
-                 parallel_scales=True, syncbn=None, parallel_branches=True, ocr_aux_rmi=False):
+                 parallel_scales=True, syncbn=None, parallel_branches=True, ocr_aux_rmi=False, init_decoder=False):
         super().__init__()
         self.arch = arch
         self.criterion = criterion
@@ -116,7 +116,9 @@ class B200SegModule(nn.Module):
         # cfg.LOSS.OCR_AUX_RMI: the auxiliary head is called with do_rmi=True (network/ocrnet.py:116,302-303); only the
         # RMILoss criterion reads do_rmi, and only the OCR architectures have an auxiliary head
         self.ocr_aux_rmi = bool(ocr_aux_rmi)
-        self.is_deepv3 = arch == "deepv3.DeepV3PlusW38"
+        self.is_deepv3 = A.has_wrn38_trunk(arch)
+        # cfg.OPTIONS.INIT_DECODER (mscale.DeepV3W38): bot_fine, bot_aspp and scale_attn get initialize_weights too
+        self.init_decoder = bool(init_decoder)
         self.hcfg = hcfg or (A.WRN38 if self.is_deepv3 else A.HRNET_W48)
         self._stem = "backbone.mod1.conv1.weight" if self.is_deepv3 else "backbone.conv1.weight"
         self.wrn_dropout_scale = 1.0     # tests set 0.0 for a dropout-free step
@@ -155,7 +157,13 @@ class B200SegModule(nn.Module):
     def _build_parameters(self):
         """Registers tensors under the reference names and reproduces its initialisation policy:
         backbone convs N(0, 1e-3), BN (1, 0) (network/hrnetv2.py:451-461); OCR / attention / seg heads keep the
-        nn.Conv2d default (kaiming_uniform(a=sqrt(5)), bias U(+-1/sqrt(fan_in))) as in network/ocrnet.py:46-83."""
+        nn.Conv2d default (kaiming_uniform(a=sqrt(5)), bias U(+-1/sqrt(fan_in))) as in network/ocrnet.py:46-83.
+        mscale.DeepV3W38 initialises only `final` (plus bot_* and scale_attn with init_decoder) with kaiming_normal_;
+        ASPP and the rest keep the nn.Conv2d default (network/mscale.py:272-278)."""
+        if self.arch == "mscale.DeepV3W38":
+            kaiming_normal = ("final", "bot_fine", "bot_aspp", "scale_attn") if self.init_decoder else ("final",)
+        else:
+            kaiming_normal = ("aspp", "bot_fine", "bot_aspp", "final")
         for name, shape, kind in self._specs:
             parts = name.split(".")
             owner = self._container(parts[:-1])
@@ -164,12 +172,12 @@ class B200SegModule(nn.Module):
             if kind == "conv_w":
                 w = torch.empty(shape)
                 if self.is_deepv3:
-                    # WRN-38 trunk: nn.Conv2d default; ASPP / bot_* / final: initialize_weights = kaiming_normal_
-                    # (network/deepv3.py:66-69, network/mynn.py:27-39)
-                    if in_backbone:
-                        nn.init.kaiming_uniform_(w, a=math.sqrt(5))
-                    else:
+                    # WRN-38 trunk: nn.Conv2d default; deepv3.DeepV3PlusW38's ASPP / bot_* / final:
+                    # initialize_weights = kaiming_normal_ (network/deepv3.py:66-69, network/mynn.py:27-39)
+                    if parts[0] in kaiming_normal:
                         nn.init.kaiming_normal_(w)
+                    else:
+                        nn.init.kaiming_uniform_(w, a=math.sqrt(5))
                 elif in_backbone:
                     nn.init.normal_(w, std=0.001)
                 else:
@@ -451,12 +459,14 @@ class B200SegModule(nn.Module):
         """Dropout2d(0.05) channel mask (network/ocr_utils.py:146) drawn from torch's generator, folded with 1/(1-p)."""
         if self.is_deepv3:
             # WRN-38 mod6 / mod7: Dropout2d(0.3) / Dropout2d(0.5) in front of conv3 (network/wider_resnet.py:302 patches
-            # nn.Dropout to Dropout2d; :336-338). One flat fp32 buffer, [n, c] per block in A.wrn_drop_layout order.
+            # nn.Dropout to Dropout2d; :336-338). One flat fp32 buffer, [n, c] per block in A.wrn_drop_layout order;
+            # the two-scale step draws a set per pass, the 0.5x pass first (network/mscale.py:188-192): [lo | hi].
             parts = []
-            for _bp, c, p in A.wrn_drop_layout(self.hcfg):
-                p = p * self.wrn_dropout_scale
-                keep = torch.bernoulli(torch.full((n * c,), 1.0 - p, dtype=F32, device=device))
-                parts.append(keep / (1.0 - p))
+            for _pass in range(2 if A.is_two_scale(self.arch) else 1):
+                for _bp, c, p in A.wrn_drop_layout(self.hcfg):
+                    p = p * self.wrn_dropout_scale
+                    keep = torch.bernoulli(torch.full((n * c,), 1.0 - p, dtype=F32, device=device))
+                    parts.append(keep / (1.0 - p))
             return torch.cat(parts) if parts else None
         if not A.has_ocr(self.arch):
             return None

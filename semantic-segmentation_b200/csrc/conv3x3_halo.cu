@@ -268,7 +268,9 @@ static int halo_smem_layout(int BN, int n_tiles, int cchunks, int cout_pad, Halo
       1024 + (2 * kMaxASlots + 2 * kMaxBSlots2) * 8 + 16 /*padding*/ + (size_t)kStatSlots * 2 * cout_pad * 4;
   const size_t resident_bytes = (size_t)9 * cchunks * b_tile;
   for (int occ = BN <= 128 ? 2 : 1; occ >= 1; --occ) {
-    const size_t budget = (occ == 2 ? kHalfSmBudget : (size_t)227 * 1024) - fixed - (size_t)smem_reserve() / occ;
+    const size_t limit = occ == 2 ? kHalfSmBudget : (size_t)227 * 1024;
+    if (fixed + (size_t)smem_reserve() / occ >= limit) continue;     // the statistics area alone does not fit
+    const size_t budget = limit - fixed - (size_t)smem_reserve() / occ;
     if (n_tiles == 1 && resident_bytes + 2 * (size_t)kASlotBytes <= budget) {
       const int as_ = (int)((budget - resident_bytes) / kASlotBytes);
       L.resident = 1; L.a_slots = as_ > kMaxASlots ? kMaxASlots : as_; L.b_slots = 0;

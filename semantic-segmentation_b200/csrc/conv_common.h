@@ -10,6 +10,7 @@ struct ConvPlan {
   int TH, TW, tiles_h, tiles_w, total_tiles, grid;
   int a_bytes, b_bytes, stage_bytes, nstages;
   int acc_regs, occ;     // fp32 accumulator registers per consumer thread (BN / 2), CTAs per SM
+  int stat_pitch, stat_window;   // statistics columns per slot in shared memory; 1: one N tile per CTA
   size_t smem_bytes;
 };
 int conv_plan(const b200seg_conv_desc* d, ConvPlan* pl);

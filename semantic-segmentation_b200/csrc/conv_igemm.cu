@@ -38,6 +38,7 @@ struct ConvKParams {
   int cchunks, KC, BN, n_tiles;
   int TH, TW, tiles_h, tiles_w, total_tiles;
   int y_ld, out_fp32, emit_stats, cout_pad, addend_ld;
+  int stat_pitch, stat_window;  // statistics columns per slot: cout_pad, or BN when each CTA keeps one N tile (below)
   int layout_type, sbo;
   int a_bytes, b_bytes, stage_bytes, nstages;
 };
@@ -55,8 +56,10 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                   float* __restrict__ stats_partials, const __nv_bfloat16* __restrict__ addend, const BnFoldDev fold) {
   static_assert(NB16 >= 1 && NB16 <= (OCC == 2 ? 8 : 16), "accumulator columns exceed the register budget");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [stages][A|B] (1024-aligned) | barriers | 16 bytes of padding | stats[kStatSlots][2][cout_pad]
-  // (the padding is part of plan_geom's byte count, which sets the ring depth)
+  // carve: [stages][A|B] (1024-aligned) | barriers | 16 bytes of padding | stats[kStatSlots][2][stat_pitch]
+  // (the padding is part of plan_geom's byte count, which sets the ring depth). stat_window: the grid is a multiple of
+  // n_tiles, so this CTA only ever sees N tile blockIdx.x % n_tiles and keeps the statistics of its BN columns only
+  // (layers too wide for a [kStatSlots][2][cout_pad] area, e.g. WideResNet-38's 4096-channel mod7).
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* stage_base = smem;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)p.nstages * p.stage_bytes);
@@ -73,8 +76,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     for (int s = 0; s < p.nstages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
     fence_barrier_init();
   }
+  const int stat_base = p.stat_window ? (int)(blockIdx.x % p.n_tiles) * p.BN : 0;   // first column of the area
   if (p.emit_stats) {
-    for (int i = threadIdx.x; i < kStatSlots * 2 * p.cout_pad; i += kThreads) s_stats[i] = 0.f;
+    for (int i = threadIdx.x; i < kStatSlots * 2 * p.stat_pitch; i += kThreads) s_stats[i] = 0.f;
   }
   __syncthreads();
   pdl_sync();   // the prologue above overlapped the previous kernel; global memory is touched only below
@@ -172,13 +176,28 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const int ho = hs * p.out_stride + p.out_off_h, wo = ws * p.out_stride + p.out_off_w;
         pix[r] = ((size_t)img * p.Ho + ho) * p.Wo + wo;
       }
-      const ConvEpi e{y, bias, addend, p.y_ld, p.addend_ld, p.out_fp32, p.Cout, p.emit_stats, p.cout_pad};
-      conv_epilogue<NB16>(acc, n_tile * p.BN, valid, pix, e, fold, smem_u32(s_stats) + warp * 8 * p.cout_pad, lane);
+      const ConvEpi e{y, bias, addend, p.y_ld, p.addend_ld, p.out_fp32, p.Cout, p.emit_stats, p.stat_pitch};
+      // the epilogue addresses column col at my_stats + 4 col: shift the base so that column stat_base lands on slot 0
+      conv_epilogue<NB16>(acc, n_tile * p.BN, valid, pix, e, fold,
+                          smem_u32(s_stats) + warp * 8 * p.stat_pitch - 4u * (uint32_t)stat_base, lane);
     }
   }
 
   __syncthreads();
-  if (p.emit_stats) {
+  if (p.emit_stats && p.stat_window) {
+    // columns outside this CTA's N tile are zero: the partials row is written whole, the cells only get the window
+    for (int i = threadIdx.x; i < 2 * p.cout_pad; i += kThreads) {
+      const int half = i / p.cout_pad, c = i - half * p.cout_pad - stat_base;
+      float v = 0.f;
+      if (c >= 0 && c < p.BN)
+        for (int s = 0; s < kStatSlots; ++s) v += s_stats[(2 * s + half) * p.stat_pitch + c];
+      if (fold.accum != nullptr) {
+        if (c >= 0 && c < p.BN) atomicAdd(fold.accum + i, (double)v);
+      } else {
+        stats_partials[(size_t)blockIdx.x * 2 * p.cout_pad + i] = v;
+      }
+    }
+  } else if (p.emit_stats) {
     if (fold.accum != nullptr) {
       bn_fold_tail(fold, s_stats, p.cout_pad);
     } else {
@@ -251,14 +270,26 @@ static int plan_geom(const LaunchGeom& g, ConvPlan* pl) {
   pl->b_bytes = pl->BN * KC * 2;
   pl->stage_bytes = (pl->a_bytes + pl->b_bytes + 1023) / 1024 * 1024;
   pl->acc_regs = pl->BN / 2;
-  size_t fixed = 1024 /*align slack*/ + 2 * kMaxStages * 8 + 16 /*padding*/ + (size_t)kStatSlots * 2 * pl->cout_pad * 4;
+  // statistics area: [kStatSlots][2][cout_pad]. A layer so wide that this area leaves no room for a two-stage ring
+  // either drops it (no statistics) or keeps only one N tile's columns per CTA (stat_window, grid a multiple of n_tiles)
+  const size_t ring_min = 2 * (size_t)pl->stage_bytes + (size_t)smem_reserve();
+  const size_t base = 1024 /*align slack*/ + 2 * kMaxStages * 8 + 16 /*padding*/;
+  pl->stat_window = 0;
+  pl->stat_pitch = pl->cout_pad;
+  if (base + (size_t)kStatSlots * 2 * pl->cout_pad * 4 + ring_min > (size_t)227 * 1024) {
+    if (g.emit_stats) pl->stat_window = 1;
+    pl->stat_pitch = g.emit_stats ? pl->BN : 0;
+  }
+  const size_t fixed = base + (size_t)kStatSlots * 2 * pl->stat_pitch * 4;
   // two CTAs per SM for narrow Cout tiles (<= 128 accumulator columns = 64 registers per consumer thread, half of the
   // shared memory each), so that CTAs of different launches overlap their fill / drain latencies on one SM; else one CTA
   // with the deepest ring
   int occ = pl->BN <= 128 ? 2 : 1;
   int nst = 0;
   for (; occ >= 1; --occ) {
-    const size_t budget = (occ == 2 ? kHalfSmBudget : (size_t)227 * 1024) - fixed - (size_t)smem_reserve() / occ;
+    const size_t limit = occ == 2 ? kHalfSmBudget : (size_t)227 * 1024;
+    if (fixed + (size_t)smem_reserve() / occ >= limit) continue;
+    const size_t budget = limit - fixed - (size_t)smem_reserve() / occ;
     nst = (int)(budget / pl->stage_bytes);
     if (nst > kMaxStages) nst = kMaxStages;
     if (nst >= (occ == 2 ? 3 : 2)) break;
@@ -272,6 +303,8 @@ static int plan_geom(const LaunchGeom& g, ConvPlan* pl) {
   {
     const int k16 = g.ntaps * pl->cchunks * (KC / 16);
     pl->grid = conv_grid_for(pl->total_tiles, slots, (double)k16 * (64.0 + pl->BN / 2));
+    if (pl->stat_window)       // every CTA keeps one N tile: tile = blockIdx.x + k * grid, n_tile = tile % n_tiles
+      pl->grid = pl->grid < pl->n_tiles ? pl->n_tiles : pl->grid / pl->n_tiles * pl->n_tiles;
   }
   return 0;
 }
@@ -420,6 +453,7 @@ static int launch_geom(const LaunchGeom& g, const void* a, const void* w, const 
   p.TH = pl.TH; p.TW = pl.TW; p.tiles_h = pl.tiles_h; p.tiles_w = pl.tiles_w; p.total_tiles = pl.total_tiles;
   p.y_ld = g.out_ld; p.out_fp32 = g.out_fp32; p.emit_stats = g.emit_stats;
   p.cout_pad = pl.cout_pad; p.addend_ld = addend_ld;
+  p.stat_pitch = pl.stat_pitch; p.stat_window = pl.stat_window;
   p.layout_type = pl.KC == 64 ? 1 : (pl.KC == 32 ? 2 : 3);   // 128B / 64B / 32B swizzle
   p.sbo = 8 * pl.KC * 2;
   p.a_bytes = pl.a_bytes; p.b_bytes = pl.b_bytes; p.stage_bytes = pl.stage_bytes; p.nstages = pl.nstages;

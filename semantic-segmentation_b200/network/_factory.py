@@ -14,8 +14,10 @@ def build(arch, num_classes, criterion):
     kw = {}
     try:
         from config import cfg
-        if not arch.startswith("deepv3."):
+        if not A.has_wrn38_trunk(arch):
             kw["hcfg"] = A.hrnet_cfg_from_reference_cfg(cfg)
+        if arch == "mscale.DeepV3W38":
+            kw["init_decoder"] = bool(getattr(getattr(cfg, "OPTIONS", None), "INIT_DECODER", False))
         ocfg = dict(A.OCR_DEFAULT)
         ocfg["mid_channels"] = cfg.MODEL.OCR.MID_CHANNELS
         ocfg["key_channels"] = cfg.MODEL.OCR.KEY_CHANNELS

@@ -1,10 +1,16 @@
-"""Overlay of the reference's network/mscale.py for the HRNet trunk (network/mscale.py:450-475): the arch string
-``mscale.HRNet`` = MscaleBasic (seg head + scale-attention head straight on the HRNet features, hierarchical two-scale
-training forward / n-scale evaluation of MscaleBase, :114-231). The DeepLab-style trunks of that file (DeeperW38 ...)
-are outside the hot path."""
+"""Overlay of the reference's network/mscale.py: the arch strings ``mscale.HRNet`` = MscaleBasic (seg head +
+scale-attention head straight on the HRNet features, :450-475) and ``mscale.DeepV3W38`` = MscaleV3Plus over the
+WideResNet-38 trunk (DeepLabV3+ decoder and scale-attention head on the same 304-channel concat, :232-336), both with
+the hierarchical two-scale training forward / n-scale evaluation of MscaleBase (:114-231). The other trunks of that
+file (ResNet-50, the fused-ASPP variants ...) are not provided."""
 from ._factory import build
 
 
 def HRNet(num_classes, criterion, s2s4=None):
     """network/mscale.py:473-475."""
     return build("mscale.HRNet", num_classes, criterion)
+
+
+def DeepV3W38(num_classes, criterion):
+    """network/mscale.py:335-336."""
+    return build("mscale.DeepV3W38", num_classes, criterion)

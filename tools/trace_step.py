@@ -114,9 +114,11 @@ def main():
             grads[n] = torch.empty(p.shape, dtype=torch.float32, device=dev)
     images = torch.empty((1, 3, args.height, args.width), dtype=torch.float32, device=dev)
     gts = torch.empty((1, args.height, args.width), dtype=torch.long, device=dev)
-    if args.arch.startswith("deepv3."):
-        from b200seg import arch as A
-        mask = torch.empty((sum(c for _b, c, _p in A.wrn_drop_layout(net.hcfg)),), dtype=torch.float32, device=dev)
+    from b200seg import arch as A
+    if A.has_wrn38_trunk(args.arch):
+        n_sets = 2 if A.is_two_scale(args.arch) else 1        # one Dropout2d mask set per scale pass
+        mask = torch.empty((n_sets * sum(c for _b, c, _p in A.wrn_drop_layout(net.hcfg)),), dtype=torch.float32,
+                           device=dev)
     else:
         mask = torch.empty((1, net.ocfg["mid_channels"]), dtype=torch.float32, device=dev)
     bncells = None
