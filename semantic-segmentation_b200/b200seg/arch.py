@@ -15,22 +15,29 @@ HRNET_W48 = dict(
     stage3=dict(num_modules=4, num_blocks=[4, 4, 4], num_channels=[48, 96, 192]),
     stage4=dict(num_modules=3, num_blocks=[4, 4, 4, 4], num_channels=[48, 96, 192, 384]),
 )
-# config.py:157-159 (OCR), :130 (SEGATTN_BOT_CH), network/ocrnet.py:63 (dropout)
-OCR_DEFAULT = dict(mid_channels=512, key_channels=256, num_classes=19, segattn_bot_ch=256, dropout=0.05)
+# config.py:157-159 (OCR), :130 (SEGATTN_BOT_CH), :131 (ASPP_BOT_CH), network/ocrnet.py:63 (dropout)
+OCR_DEFAULT = dict(mid_channels=512, key_channels=256, num_classes=19, segattn_bot_ch=256, dropout=0.05,
+                   aspp_bot_ch=256)
 
 ARCHS = ("ocrnet.HRNet_Mscale", "ocrnet.HRNet", "basic.HRNet", "mscale.HRNet", "deepv3.DeepV3PlusW38",
-         "mscale.DeepV3W38")
+         "mscale.DeepV3W38", "basic.HRNet_ASP", "mscale.HRNet_ASP")
 
 
 def is_two_scale(arch):
     """Architectures whose training forward is the hierarchical two-scale pass (MscaleOCR.two_scale_forward,
     network/ocrnet.py:264-334; MscaleBase.two_scale_forward, network/mscale.py:182-231)."""
-    return arch in ("ocrnet.HRNet_Mscale", "mscale.HRNet", "mscale.DeepV3W38")
+    return arch in ("ocrnet.HRNet_Mscale", "mscale.HRNet", "mscale.DeepV3W38", "mscale.HRNet_ASP")
 
 
 def has_wrn38_trunk(arch):
     """Architectures built on the WideResNet-38 trunk, ASPP and 304-channel decoder (DeepV3Plus, MscaleV3Plus)."""
     return arch in ("deepv3.DeepV3PlusW38", "mscale.DeepV3W38")
+
+
+def has_hrnet_aspp(arch):
+    """Architectures with the ASPP over the HRNet trunk's stride-4 features (basic.ASPP, network/basic.py:67-101;
+    mscale.ASPP, network/mscale.py:479-511)."""
+    return arch in ("basic.HRNet_ASP", "mscale.HRNet_ASP")
 
 
 def has_ocr(arch):
@@ -64,6 +71,15 @@ def wrn_drop_layout(wcfg=WRN38):
             if drop is not None and len(ch) == 3]
 
 
+def aspp_specs(conv, bn, high, red):
+    """AtrousSpatialPyramidPoolingModule.__init__ (network/utils.py:174-205): the 1x1 and dilated 3x3 branches
+    (`features`), then the image-pooling branch, each `red` (bottleneck_ch) wide over `high` input channels."""
+    conv("aspp.features.0.0", red, high, 1); bn("aspp.features.0.1", red)
+    for i in range(len(ASPP_RATES)):
+        conv("aspp.features.%d.0" % (i + 1), red, high, 3); bn("aspp.features.%d.1" % (i + 1), red)
+    conv("aspp.img_conv.0", red, high, 1); bn("aspp.img_conv.1", red)
+
+
 def deepv3_tensor_specs(num_classes=19, wcfg=WRN38, bot_ch=256, scale_attn=False):
     """(name, shape, kind) of deepv3.DeepV3PlusW38 in the reference's registration order (network/deepv3.py:46-65,
     network/utils.py:171-202). scale_attn: mscale.DeepV3W38 (MscaleV3Plus.__init__, network/mscale.py:236-277), whose
@@ -95,10 +111,7 @@ def deepv3_tensor_specs(num_classes=19, wcfg=WRN38, bot_ch=256, scale_attn=False
         if stride != 1 or in_ch != ch[-1]:
             conv(b + ".proj_conv", ch[-1], in_ch, 1)
     high, s2_ch = wcfg["channels"][-1][-1], wcfg["channels"][0][-1]
-    conv("aspp.features.0.0", 256, high, 1); bn("aspp.features.0.1", 256)
-    for i in range(len(ASPP_RATES)):
-        conv("aspp.features.%d.0" % (i + 1), 256, high, 3); bn("aspp.features.%d.1" % (i + 1), 256)
-    conv("aspp.img_conv.0", 256, high, 1); bn("aspp.img_conv.1", 256)
+    aspp_specs(conv, bn, high, 256)
     conv("bot_fine", 48, s2_ch, 1)
     conv("bot_aspp", 256, 256 * (2 + len(ASPP_RATES)), 1)
     conv("final.0", bot_ch, 256 + 48, 3); bn("final.1", bot_ch)
@@ -219,6 +232,21 @@ def tensor_specs(arch, hcfg=HRNET_W48, ocfg=OCR_DEFAULT):
         conv(s + ".0", bot, high, 3); bn(s + ".1", bot)
         conv(s + ".3", bot, bot, 3); bn(s + ".4", bot)
         conv(s + ".6", ncls, bot, 1)
+    elif has_hrnet_aspp(arch):
+        # basic.ASPP / mscale.ASPP.__init__ (network/basic.py:71-82, network/mscale.py:483-494): get_aspp(720,
+        # ASPP_BOT_CH) -> bot_aspp (1x1 to 256, no bias) -> final = make_seg_head(256) [-> scale_attn =
+        # make_attn_head(256)]
+        red, bot, ncls = ocfg["aspp_bot_ch"], ocfg["segattn_bot_ch"], ocfg["num_classes"]
+        aspp_specs(conv, bn, high, red)
+        conv("bot_aspp", 256, red * (2 + len(ASPP_RATES)), 1)
+        conv("final.0", bot, 256, 3); bn("final.1", bot)
+        conv("final.3", bot, bot, 3); bn("final.4", bot)
+        conv("final.6", ncls, bot, 1)
+        if arch == "mscale.HRNet_ASP":
+            a = "scale_attn"
+            conv(a + ".conv0", bot, 256, 3); bn(a + ".bn0", bot)
+            conv(a + ".conv1", bot, bot, 3); bn(a + ".bn1", bot)
+            conv(a + ".conv2", 1, bot, 1)
     elif arch == "mscale.HRNet":
         # MscaleBasic.__init__ (network/mscale.py:450-461): backbone, cls_head = make_seg_head, scale_attn = make_attn_head
         bot, ncls = ocfg["segattn_bot_ch"], ocfg["num_classes"]

@@ -5,8 +5,10 @@ reference's output assembly in fp32 NCHW on the device.
                         eval branch of two_scale_forward (:264-327)
   mscale.HRNet        : MscaleBase.nscale_forward / two_scale_forward eval branches (network/mscale.py:114-231)
   mscale.DeepV3W38    : the same assembly over the WRN-38 / ASPP / decoder pass (MscaleV3Plus._fwd, :296-328)
+  mscale.HRNet_ASP    : the same assembly over the HRNet / ASPP pass (mscale.ASPP._fwd, :496-511)
   ocrnet.HRNet        : OCRNet.forward eval branch (:104-122)
   basic.HRNet         : Basic.forward eval branch (network/basic.py:50-64)
+  basic.HRNet_ASP     : ASPP.forward eval branch (network/basic.py:84-101)
   deepv3.DeepV3PlusW38: DeepV3Plus.forward eval branch (network/deepv3.py:73-96)
 """
 import torch

@@ -16,7 +16,7 @@ def eval_minibatch(net, images, gts, scales=(1.0,), do_flip=False, mscale=None, 
     Returns dict(predictions int64 [N,H,W], prob_mask fp32 [N,H,W], hist int64 [19,19] accumulated into ``hist``)."""
     assert not net.training
     if mscale is None:
-        mscale = net.arch in ("ocrnet.HRNet_Mscale", "mscale.HRNet") and bool(net.n_scales)
+        mscale = net.arch in ("ocrnet.HRNet_Mscale", "mscale.HRNet", "mscale.HRNet_ASP") and bool(net.n_scales)
     if mscale:
         scales = (1.0,)
     n, _, H, W = images.shape

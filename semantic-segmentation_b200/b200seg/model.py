@@ -249,6 +249,24 @@ def wrn_block(E, p, x, in_ch, ch, stride, dil, drop_mask):
     return E.conv_sum(t, c + ".conv3", 1, 1, 1, addend=short, want_stats=True)
 
 
+def aspp(E, x, red):
+    """AtrousSpatialPyramidPoolingModule.forward (network/utils.py:207-218) at output stride 8 (rates 12 / 24 / 36):
+    image pooling, the 1x1 and the three dilated 3x3 branches, each `red` channels wide, written into their slices of
+    one concat Act [n, h, w, 5 * red] = [img | 1x1 | d12 | d24 | d36]."""
+    n, h, w, _ = x.t.shape
+    cat = Act(raw._new((n, h, w, 5 * red), dtype=BF16, device=x.t.device))
+    img = E.conv_bn(E.image_pool(x), "aspp.img_conv.0", "aspp.img_conv.1", 1)
+    pieces = [(E.broadcast(img, h, w, cat.t[..., 0:red]), 0, red)]
+    one = E.conv_bn(x, "aspp.features.0.0", "aspp.features.0.1", 1, out=cat.t[..., red:2 * red])
+    pieces.append((one, red, 2 * red))
+    for i, r in enumerate(A.ASPP_RATES):
+        c0 = (2 + i) * red
+        f = "aspp.features.%d" % (i + 1)
+        pieces.append((E.conv_bn(x, f + ".0", f + ".1", 3, dilation=r, out=cat.t[..., c0:c0 + red]), c0, c0 + red))
+    E.slice_marker(cat, pieces)
+    return cat
+
+
 def deepv3_pass(E, images, wcfg, size_hw, drop_mask):
     """DeepV3Plus.forward up to the half-resolution logits (network/deepv3.py:75-88), MscaleV3Plus._fwd up to its two
     heads (network/mscale.py:296-316): WRN-38 trunk (output stride 8), ASPP (network/utils.py:204-216), decoder.
@@ -274,17 +292,7 @@ def deepv3_pass(E, images, wcfg, size_hw, drop_mask):
         feats[mod] = x
     s2, final = feats["mod2"], x
     dev = final.t.device
-    h8, w8 = final.t.shape[1:3]
-    cat = Act(raw._new((n, h8, w8, 5 * 256), dtype=BF16, device=dev))      # [img | 1x1 | d12 | d24 | d36]
-    img = E.conv_bn(E.image_pool(final), "aspp.img_conv.0", "aspp.img_conv.1", 1)
-    pieces = [(E.broadcast(img, h8, w8, cat.t[..., 0:256]), 0, 256)]
-    pieces.append((E.conv_bn(final, "aspp.features.0.0", "aspp.features.0.1", 1, out=cat.t[..., 256:512]), 256, 512))
-    for i, r in enumerate(A.ASPP_RATES):
-        c0 = 512 + 256 * i
-        f = "aspp.features.%d" % (i + 1)
-        pieces.append((E.conv_bn(final, f + ".0", f + ".1", 3, dilation=r, out=cat.t[..., c0:c0 + 256]), c0, c0 + 256))
-    E.slice_marker(cat, pieces)
-    conv_aspp = E.conv_sum(cat, "bot_aspp", 1)
+    conv_aspp = E.conv_sum(aspp(E, final, 256), "bot_aspp", 1)
     h2, w2 = s2.t.shape[1:3]
     cat2 = Act(raw._new((n, h2, w2, 48 + 256), dtype=BF16, device=dev))
     conv_s2 = E.conv_sum(s2, "bot_fine", 1, out=cat2.t[..., :48])
@@ -300,12 +308,20 @@ def scale_pass(E, images, size_hw, arch, hcfg, ocfg, drop_mask=None):
     """MscaleOCR._fwd (network/ocrnet.py:170-183) up to the quarter-resolution maps (the x4 Upsample is fused into the
     blend/loss kernels). images: fp32 NCHW; size_hw: pass input size (ResizeX folded into image_prep).
     mscale.DeepV3W38: MscaleV3Plus._fwd (network/mscale.py:296-328) up to the half-resolution maps; drop_mask: this
-    pass' WRN-38 Dropout2d multipliers (deepv3_pass)."""
+    pass' WRN-38 Dropout2d multipliers (deepv3_pass). basic.HRNet_ASP / mscale.HRNet_ASP: the ASPP models over the
+    HRNet trunk, up to their quarter-resolution maps."""
     if arch == "mscale.DeepV3W38":     # both heads read the decoder concat
         cls, cat = deepv3_pass(E, images, hcfg, size_hw, drop_mask)
         return dict(cls=cls, aux=None, attn=attn_head(E, cat))
     x16 = Act(raw.image_prep(images, size_hw[0], size_hw[1]), needs_grad=False)
     feats = hrnet_forward(E, x16, hcfg)
+    if A.has_hrnet_aspp(arch):
+        # basic.ASPP.forward / mscale.ASPP._fwd (network/basic.py:84-92, network/mscale.py:496-511): ASPP on the
+        # stride-4 trunk features, bot_aspp (1x1, no BN / ReLU), then the seg head and, for the mscale model, the
+        # attention head on the same 256-channel map
+        x = E.conv_sum(aspp(E, feats, ocfg["aspp_bot_ch"]), "bot_aspp", 1)
+        cls = seg_head(E, x, "final")
+        return dict(cls=cls, aux=None, attn=attn_head(E, x) if arch == "mscale.HRNet_ASP" else None)
     if arch == "basic.HRNet":
         return dict(cls=seg_head(E, feats), aux=None, attn=None)
     if arch == "mscale.HRNet":      # MscaleBasic._fwd (network/mscale.py:463-470): both heads read the trunk features
@@ -318,10 +334,11 @@ def scale_pass(E, images, size_hw, arch, hcfg, ocfg, drop_mask=None):
 def train_loss(E, images, gts, arch, hcfg, ocfg, lo_scale=0.5, ocr_alpha=0.4, sup_wt=0.0, ignore_index=255, E_lo=None,
                loss_kind="ce", img_wt=(1.0, False), ocr_aux_rmi=False):
     """Training forward + loss. ocrnet.HRNet_Mscale: MscaleOCR.two_scale_forward (network/ocrnet.py:264-319);
-    mscale.HRNet, mscale.DeepV3W38: MscaleBase.two_scale_forward (network/mscale.py:182-220; one head, no auxiliary
-    loss; the DeepLab model's maps are on the half-resolution grid of each pass); deepv3.DeepV3PlusW38:
-    DeepV3Plus.forward (network/deepv3.py:73-96);
-    ocrnet.HRNet: OCRNet.forward (:104-122); basic.HRNet: Basic.forward (network/basic.py:50-64).
+    mscale.HRNet, mscale.DeepV3W38, mscale.HRNet_ASP: MscaleBase.two_scale_forward (network/mscale.py:182-220; one
+    head, no auxiliary loss; the DeepLab model's maps are on the half-resolution grid of each pass);
+    deepv3.DeepV3PlusW38: DeepV3Plus.forward (network/deepv3.py:73-96);
+    ocrnet.HRNet: OCRNet.forward (:104-122); basic.HRNet: Basic.forward (network/basic.py:50-64); basic.HRNet_ASP:
+    ASPP.forward (network/basic.py:84-101).
     Returns the fp32 loss vector [total, cls, aux, sup_lo, sup_hi, rmi, aux rmi, 0]; pushes the loss backward on the
     tape. loss_kind "ce": CrossEntropyLoss2d (loss/utils.py:133-134); "rmi": RMILoss (loss/rmi.py:70-215) = sigmoid BCE
     on every head (the auxiliary / supervised terms are called with do_rmi=False, network/ocrnet.py:303-318) plus the

@@ -124,8 +124,15 @@ class B200SegModule(nn.Module):
         self.wrn_dropout_scale = 1.0     # tests set 0.0 for a dropout-free step
         self.ocfg = dict(ocfg or A.OCR_DEFAULT)
         self.ocfg["num_classes"] = num_classes
+        self.ocfg.setdefault("aspp_bot_ch", A.OCR_DEFAULT["aspp_bot_ch"])
         if num_classes != 19:
             raise NotImplementedError("the loss / soft-region kernels are instantiated for the 19 Cityscapes classes")
+        red = self.ocfg["aspp_bot_ch"]
+        if A.has_hrnet_aspp(arch) and (red <= 0 or red % 16):
+            # bot_aspp reads the 5 * red channel concat: the weight-gradient GEMM takes input widths in whole
+            # 16-channel groups (csrc/wgrad_igemm.cu)
+            raise NotImplementedError("cfg.MODEL.ASPP_BOT_CH must be a positive multiple of 16 on the sm_90a "
+                                      "convolutions; got %d" % red)
         self.lo_scale, self.ocr_alpha, self.sup_wt, self.ignore_index = lo_scale, ocr_alpha, supervised_mscale_wt, ignore_index
         self.n_scales = n_scales
         self.use_cuda_graph = use_cuda_graph
@@ -159,11 +166,16 @@ class B200SegModule(nn.Module):
         backbone convs N(0, 1e-3), BN (1, 0) (network/hrnetv2.py:451-461); OCR / attention / seg heads keep the
         nn.Conv2d default (kaiming_uniform(a=sqrt(5)), bias U(+-1/sqrt(fan_in))) as in network/ocrnet.py:46-83.
         mscale.DeepV3W38 initialises only `final` (plus bot_* and scale_attn with init_decoder) with kaiming_normal_;
-        ASPP and the rest keep the nn.Conv2d default (network/mscale.py:272-278)."""
+        ASPP and the rest keep the nn.Conv2d default (network/mscale.py:272-278). basic.HRNet_ASP initialises `final`,
+        `bot_aspp` and `aspp` (network/basic.py:82), mscale.HRNet_ASP only `final` (network/mscale.py:494)."""
         if self.arch == "mscale.DeepV3W38":
             kaiming_normal = ("final", "bot_fine", "bot_aspp", "scale_attn") if self.init_decoder else ("final",)
-        else:
+        elif self.arch == "mscale.HRNet_ASP":
+            kaiming_normal = ("final",)
+        elif self.is_deepv3 or self.arch == "basic.HRNet_ASP":
             kaiming_normal = ("aspp", "bot_fine", "bot_aspp", "final")
+        else:
+            kaiming_normal = ()
         for name, shape, kind in self._specs:
             parts = name.split(".")
             owner = self._container(parts[:-1])
@@ -171,13 +183,12 @@ class B200SegModule(nn.Module):
             in_backbone = parts[0] == "backbone"
             if kind == "conv_w":
                 w = torch.empty(shape)
-                if self.is_deepv3:
-                    # WRN-38 trunk: nn.Conv2d default; deepv3.DeepV3PlusW38's ASPP / bot_* / final:
+                if parts[0] in kaiming_normal:
                     # initialize_weights = kaiming_normal_ (network/deepv3.py:66-69, network/mynn.py:27-39)
-                    if parts[0] in kaiming_normal:
-                        nn.init.kaiming_normal_(w)
-                    else:
-                        nn.init.kaiming_uniform_(w, a=math.sqrt(5))
+                    nn.init.kaiming_normal_(w)
+                elif self.is_deepv3:
+                    # WRN-38 trunk and the layers initialize_weights leaves alone: nn.Conv2d default
+                    nn.init.kaiming_uniform_(w, a=math.sqrt(5))
                 elif in_backbone:
                     nn.init.normal_(w, std=0.001)
                 else:

@@ -22,6 +22,8 @@ def build(arch, num_classes, criterion):
         ocfg["mid_channels"] = cfg.MODEL.OCR.MID_CHANNELS
         ocfg["key_channels"] = cfg.MODEL.OCR.KEY_CHANNELS
         ocfg["segattn_bot_ch"] = cfg.MODEL.SEGATTN_BOT_CH
+        if A.has_hrnet_aspp(arch):
+            ocfg["aspp_bot_ch"] = int(cfg.MODEL.ASPP_BOT_CH)      # --aspp_bot_ch (config.py:131,313)
         kw["ocfg"] = ocfg
         kw["lo_scale"] = cfg.MODEL.MSCALE_LO_SCALE
         kw["ocr_alpha"] = cfg.LOSS.OCR_ALPHA
