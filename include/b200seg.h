@@ -254,22 +254,27 @@ int b200seg_accum_f32(float* dst, const float* src, int64_t n, void* stream);
  * 1 / world_size of the data-parallel average (network/__init__.py:38-39 apex DDP). */
 int b200seg_publish_grads(float* dst, const float* src, int64_t n, const float* scale_dev, float scale_const,
                           int32_t accumulate, void* stream);
-/* z = relu?(y*scale + shift [+ res]) [* post_scale[n][c]]   (post_scale carries the Dropout2d mask/(1-p),
- * network/ocr_utils.py:146). npix = n*h*w, hw = h*w. */
+/* z = relu?(y*scale + shift [+ res]) [* post_scale[n][c]] [* 2 keep]   (post_scale carries the Dropout2d mask/(1-p),
+ * network/ocr_utils.py:146). npix = n*h*w, hw = h*w.
+ * drop_seed (device pointer to one uint64, may be NULL = off): element-wise Dropout(0.5), network/utils.py:359-360.
+ * The keep bit of element i = pixel * c + channel is bit i % 128 of Philox4x32-10(counter {i / 128, drop_pass, 0},
+ * key *drop_seed); nothing is stored, the backward entry points below regenerate the same bits from the same
+ * (drop_seed, drop_pass). drop_pass separates the scale passes of one step. */
 int b200seg_bn_apply(const void* y, int32_t y_ld, const float* scale, const float* shift, const void* res,
                      int32_t res_ld, const float* post_scale, int32_t relu, void* z, int32_t z_ld, int64_t npix,
-                     int32_t hw, int32_t c, void* stream);
+                     int32_t hw, int32_t c, const uint64_t* drop_seed, int32_t drop_pass, void* stream);
 /* The same pass as the consumer of a convolution launched with b200seg_conv2d_fwd_bn: every block derives scale / shift
  * from f->accum (fp64 [2][roundup16(c)] sums), block 0 writes f->scale / shift / mean / invstd (+ batch or running
  * statistics exactly like b200seg_bn_finalize). */
 int b200seg_bn_apply_cells(const void* y, int32_t y_ld, const b200seg_bn_fold* f, const void* res, int32_t res_ld,
                            const float* post_scale, int32_t relu, void* z, int32_t z_ld, int64_t npix, int32_t hw,
-                           int32_t c, void* stream);
-/* backward: g = dz * post_scale * (mask > 0); partials[grid][2][c] of (sum g, sum g*xhat), grid from _bn_bwd_grid */
+                           int32_t c, const uint64_t* drop_seed, int32_t drop_pass, void* stream);
+/* backward: g = dz * post_scale [* 2 keep] * (mask > 0); partials[grid][2][c] of (sum g, sum g*xhat), grid from
+ * _bn_bwd_grid. drop_seed / drop_pass: those of the forward apply pass (NULL = no dropout). */
 int32_t b200seg_bn_bwd_grid(int64_t npix, int32_t c);
 int b200seg_bn_bwd_reduce(const void* dz, int32_t dz_ld, const void* mask, int32_t mask_ld, const float* post_scale,
                           const void* y, int32_t y_ld, const float* mean, const float* invstd, int64_t npix, int32_t hw,
-                          int32_t c, float* partials, void* stream);
+                          int32_t c, float* partials, const uint64_t* drop_seed, int32_t drop_pass, void* stream);
 /* dgamma += sum g*xhat, dbeta += sum g (accumulating), c1 = sum g / count, c2 = sum g*xhat / count */
 int b200seg_bn_bwd_finalize(const float* partials, int32_t grid, int32_t c, float count, float* dgamma, float* dbeta,
                             float* c1, float* c2, const b200seg_bn_sync* sync, void* stream);
@@ -277,14 +282,16 @@ int b200seg_bn_bwd_finalize(const float* partials, int32_t grid, int32_t c, floa
 int b200seg_bn_bwd_apply(const void* dz, int32_t dz_ld, const void* mask, int32_t mask_ld, const float* post_scale,
                          const void* y, int32_t y_ld, const float* mean, const float* invstd, const float* gamma,
                          const float* c1, const float* c2, void* dy, int32_t dy_ld, void* g_out, int32_t g_ld,
-                         int32_t g_accumulate, int64_t npix, int32_t hw, int32_t c, void* stream);
+                         int32_t g_accumulate, int64_t npix, int32_t hw, int32_t c, const uint64_t* drop_seed,
+                         int32_t drop_pass, void* stream);
 /* reduce + gradient pass with deferred finalisation (two launches): the reduction adds its sums to cells ([2][c] fp64,
  * zeroed by the caller once per step), the gradient pass folds them in its prologue and accumulates dgamma / dbeta
  * (either may be NULL). Per-GPU statistics only (SyncBN: _reduce + _finalize + _apply). */
 int b200seg_bn_bwd_cells(const void* dz, int32_t dz_ld, const void* mask, int32_t mask_ld, const float* post_scale,
                          const void* y, int32_t y_ld, const float* mean, const float* invstd, const float* gamma,
                          float* dgamma, float* dbeta, double* cells, void* dy, int32_t dy_ld, void* g_out, int32_t g_ld,
-                         int32_t g_accumulate, int64_t npix, int32_t hw, int32_t c, void* stream);
+                         int32_t g_accumulate, int64_t npix, int32_t hw, int32_t c, const uint64_t* drop_seed,
+                         int32_t drop_pass, void* stream);
 /* dst (=|+=) src * (mask > 0) */
 int b200seg_masked_accum(const void* src, int32_t src_ld, const void* mask, int32_t mask_ld, void* dst, int32_t dst_ld,
                          int32_t accumulate, int64_t npix, int32_t c, void* stream);

@@ -101,15 +101,16 @@ SIGNATURES = {
     "b200seg_publish_grads": (ctypes.c_int, [V, V, I64, V, F, I32, V]),
     "b200seg_sgd_chunk": (I32, []),
     "b200seg_sgd_step": (ctypes.c_int, [V, V, V, I32, F, F, F, F, I32, I32, V]),
-    "b200seg_bn_apply": (ctypes.c_int, [V, I32, V, V, V, I32, V, I32, V, I32, I64, I32, I32, V]),
-    "b200seg_bn_apply_cells": (ctypes.c_int, [V, I32, ctypes.POINTER(BnFold), V, I32, V, I32, V, I32, I64, I32, I32, V]),
+    "b200seg_bn_apply": (ctypes.c_int, [V, I32, V, V, V, I32, V, I32, V, I32, I64, I32, I32, V, I32, V]),
+    "b200seg_bn_apply_cells": (ctypes.c_int, [V, I32, ctypes.POINTER(BnFold), V, I32, V, I32, V, I32, I64, I32, I32, V,
+                                              I32, V]),
     "b200seg_bn_bwd_grid": (I32, [I64, I32]),
-    "b200seg_bn_bwd_reduce": (ctypes.c_int, [V, I32, V, I32, V, V, I32, V, V, I64, I32, I32, V, V]),
+    "b200seg_bn_bwd_reduce": (ctypes.c_int, [V, I32, V, I32, V, V, I32, V, V, I64, I32, I32, V, V, I32, V]),
     "b200seg_bn_bwd_finalize": (ctypes.c_int, [V, I32, I32, F, V, V, V, V, ctypes.POINTER(BnSync), V]),
     "b200seg_bn_bwd_apply": (ctypes.c_int, [V, I32, V, I32, V, V, I32, V, V, V, V, V, V, I32, V, I32, I32, I64, I32,
-                                            I32, V]),
+                                            I32, V, I32, V]),
     "b200seg_bn_bwd_cells": (ctypes.c_int, [V, I32, V, I32, V, V, I32, V, V, V, V, V, V, V, I32, V, I32, I32, I64, I32,
-                                            I32, V]),
+                                            I32, V, I32, V]),
     "b200seg_masked_accum": (ctypes.c_int, [V, I32, V, I32, V, I32, I32, I64, I32, V]),
     "b200seg_fuse_fwd": (ctypes.c_int, [ctypes.POINTER(FuseDesc), V, I32, V]),
     "b200seg_upsample_adjoint": (ctypes.c_int, [V, I32, V, I32, I32, I32, I32, I32, V, I32, I32, I32, I32, V]),
@@ -154,6 +155,7 @@ SIGNATURES = {
 # test-only entry points (csrc/probe.h, libb200seg_test.so), not part of include/b200seg.h / the product library
 PROBE_SIGNATURES = {
     "b200seg_conv2d_fwd_direct": (ctypes.c_int, [ctypes.POINTER(ConvDesc), V, V, V, V, V]),
+    "b200seg_dropout_keep_mask": (ctypes.c_int, [V, I32, I64, I32, V, V]),
 }
 
 _lib = None

@@ -15,9 +15,10 @@ HRNET_W48 = dict(
     stage3=dict(num_modules=4, num_blocks=[4, 4, 4], num_channels=[48, 96, 192]),
     stage4=dict(num_modules=3, num_blocks=[4, 4, 4, 4], num_channels=[48, 96, 192, 384]),
 )
-# config.py:157-159 (OCR), :130 (SEGATTN_BOT_CH), :131 (ASPP_BOT_CH), network/ocrnet.py:63 (dropout)
+# config.py:157-159 (OCR), :130 (SEGATTN_BOT_CH), :131 (ASPP_BOT_CH), network/ocrnet.py:63 (dropout),
+# :133-135 (MSCALE_INNER_3x3 / MSCALE_DROPOUT / MSCALE_OLDARCH: --mscale_no3x3 / --mscale_dropout / --mscale_old_arch)
 OCR_DEFAULT = dict(mid_channels=512, key_channels=256, num_classes=19, segattn_bot_ch=256, dropout=0.05,
-                   aspp_bot_ch=256)
+                   aspp_bot_ch=256, mscale_inner_3x3=True, mscale_dropout=False, mscale_oldarch=False)
 
 ARCHS = ("ocrnet.HRNet_Mscale", "ocrnet.HRNet", "basic.HRNet", "mscale.HRNet", "deepv3.DeepV3PlusW38",
          "mscale.DeepV3W38", "basic.HRNet_ASP", "mscale.HRNet_ASP")
@@ -80,11 +81,34 @@ def aspp_specs(conv, bn, high, red):
     conv("aspp.img_conv.0", red, high, 1); bn("aspp.img_conv.1", red)
 
 
-def deepv3_tensor_specs(num_classes=19, wcfg=WRN38, bot_ch=256, scale_attn=False):
+def attn_head_plan(ocfg, p="scale_attn"):
+    """The attention head the cfg selects: ([(conv, bn) of each 3x3 conv + BN + ReLU stage], final 1x1 conv,
+    whether nn.Dropout(0.5) sits in front of it).
+    make_attn_head (network/utils.py:343-367): conv0/bn0, conv1/bn1 unless MSCALE_INNER_3x3 is off, `drop` when
+    MSCALE_DROPOUT is on, conv2. old_make_attn_head (:370-382, MSCALE_OLDARCH, which ignores the other two keys): the
+    same two stages and 1x1 conv as an unnamed nn.Sequential (0/1/3/4/6)."""
+    if ocfg.get("mscale_oldarch", False):
+        return [(p + ".0", p + ".1"), (p + ".3", p + ".4")], p + ".6", False
+    stages = [(p + ".conv0", p + ".bn0")]
+    if ocfg.get("mscale_inner_3x3", True):
+        stages.append((p + ".conv1", p + ".bn1"))
+    return stages, p + ".conv2", bool(ocfg.get("mscale_dropout", False))
+
+
+def attn_head_specs(conv, bn, in_ch, bot, ocfg):
+    """Parameters of the attention head over `in_ch` input channels, `bot` (cfg.MODEL.SEGATTN_BOT_CH) wide, in the
+    reference's registration order."""
+    stages, last, _drop = attn_head_plan(ocfg)
+    for i, (c, b) in enumerate(stages):
+        conv(c, bot, in_ch if i == 0 else bot, 3); bn(b, bot)
+    conv(last, 1, bot, 1)
+
+
+def deepv3_tensor_specs(num_classes=19, wcfg=WRN38, bot_ch=256, scale_attn=False, ocfg=OCR_DEFAULT):
     """(name, shape, kind) of deepv3.DeepV3PlusW38 in the reference's registration order (network/deepv3.py:46-65,
     network/utils.py:171-202). scale_attn: mscale.DeepV3W38 (MscaleV3Plus.__init__, network/mscale.py:236-277), whose
     decoder `final` is bot_ch (cfg.MODEL.SEGATTN_BOT_CH) wide and is followed by the attention head on the same
-    304-channel concat."""
+    304-channel concat, in the variant ocfg selects (attn_head_plan)."""
     out = []
 
     def conv(name, o, i, k):
@@ -117,10 +141,8 @@ def deepv3_tensor_specs(num_classes=19, wcfg=WRN38, bot_ch=256, scale_attn=False
     conv("final.0", bot_ch, 256 + 48, 3); bn("final.1", bot_ch)
     conv("final.3", bot_ch, bot_ch, 3); bn("final.4", bot_ch)
     conv("final.6", num_classes, bot_ch, 1)
-    if scale_attn:      # make_attn_head(304, 1) (network/utils.py:343-367)
-        conv("scale_attn.conv0", bot_ch, 256 + 48, 3); bn("scale_attn.bn0", bot_ch)
-        conv("scale_attn.conv1", bot_ch, bot_ch, 3); bn("scale_attn.bn1", bot_ch)
-        conv("scale_attn.conv2", 1, bot_ch, 1)
+    if scale_attn:      # make_attn_head(304, 1)
+        attn_head_specs(conv, bn, 256 + 48, bot_ch, ocfg)
     return out
 
 
@@ -144,7 +166,7 @@ def tensor_specs(arch, hcfg=HRNET_W48, ocfg=OCR_DEFAULT):
         return deepv3_tensor_specs(ocfg["num_classes"], hcfg if "structure" in hcfg else WRN38)
     if arch == "mscale.DeepV3W38":
         return deepv3_tensor_specs(ocfg["num_classes"], hcfg if "structure" in hcfg else WRN38,
-                                   ocfg["segattn_bot_ch"], scale_attn=True)
+                                   ocfg["segattn_bot_ch"], scale_attn=True, ocfg=ocfg)
     out = []
 
     def conv(name, o, i, k, bias=False):
@@ -221,11 +243,7 @@ def tensor_specs(arch, hcfg=HRNET_W48, ocfg=OCR_DEFAULT):
         conv(o + ".aux_head.0", high, high, 1, True); bn(o + ".aux_head.1.0", high)
         conv(o + ".aux_head.2", ncls, high, 1, True)
         if arch == "ocrnet.HRNet_Mscale":
-            bot = ocfg["segattn_bot_ch"]
-            a = "scale_attn"
-            conv(a + ".conv0", bot, mid, 3); bn(a + ".bn0", bot)
-            conv(a + ".conv1", bot, bot, 3); bn(a + ".bn1", bot)
-            conv(a + ".conv2", 1, bot, 1)
+            attn_head_specs(conv, bn, mid, ocfg["segattn_bot_ch"], ocfg)
     elif arch == "basic.HRNet":
         bot, ncls = ocfg["segattn_bot_ch"], ocfg["num_classes"]
         s = "seg_head"
@@ -243,10 +261,7 @@ def tensor_specs(arch, hcfg=HRNET_W48, ocfg=OCR_DEFAULT):
         conv("final.3", bot, bot, 3); bn("final.4", bot)
         conv("final.6", ncls, bot, 1)
         if arch == "mscale.HRNet_ASP":
-            a = "scale_attn"
-            conv(a + ".conv0", bot, 256, 3); bn(a + ".bn0", bot)
-            conv(a + ".conv1", bot, bot, 3); bn(a + ".bn1", bot)
-            conv(a + ".conv2", 1, bot, 1)
+            attn_head_specs(conv, bn, 256, bot, ocfg)
     elif arch == "mscale.HRNet":
         # MscaleBasic.__init__ (network/mscale.py:450-461): backbone, cls_head = make_seg_head, scale_attn = make_attn_head
         bot, ncls = ocfg["segattn_bot_ch"], ocfg["num_classes"]
@@ -254,10 +269,7 @@ def tensor_specs(arch, hcfg=HRNET_W48, ocfg=OCR_DEFAULT):
         conv(s + ".0", bot, high, 3); bn(s + ".1", bot)
         conv(s + ".3", bot, bot, 3); bn(s + ".4", bot)
         conv(s + ".6", ncls, bot, 1)
-        a = "scale_attn"
-        conv(a + ".conv0", bot, high, 3); bn(a + ".bn0", bot)
-        conv(a + ".conv1", bot, bot, 3); bn(a + ".bn1", bot)
-        conv(a + ".conv2", 1, bot, 1)
+        attn_head_specs(conv, bn, high, bot, ocfg)
     else:
         raise ValueError("unsupported arch %r (hot path covers %s)" % (arch, ", ".join(ARCHS)))
     return out

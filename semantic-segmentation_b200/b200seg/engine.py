@@ -52,7 +52,7 @@ class HeadRec:
 
 class Engine:
     def __init__(self, params, grads, packed, training, drop_mask=None, side_stream=None, bstat=None, stream=None,
-                 sync=None, pass_id=0, branch_streams=None, ws_holder=None, bncells=None):
+                 sync=None, pass_id=0, branch_streams=None, ws_holder=None, bncells=None, attn_seed=None):
         """params: name -> tensor (weights, BN buffers); grads: name -> fp32 tensor accumulated into (training);
         packed: name -> (w_fwd, w_dgrad) bf16 operand caches; drop_mask: fp32 [N, mid] post-ReLU multiplier;
         bstat: BN layer name -> fp32 [2*C] slot receiving the batch [mean | unbiased var] (the running statistics are
@@ -64,12 +64,14 @@ class Engine:
         of the step: deferred finalisation - the convolution / the backward reduction only add their sums to the cells
         and the consuming apply pass folds them in its prologue (no finaliser launch on the chain; ignored with sync);
         branch_streams: up to three extra streams for the parallel branches of a HighResolutionModule (branch 0 stays
-        on the engine's own stream); ws_holder: reusable weight-gradient slab workspace of the side stream."""
+        on the engine's own stream); ws_holder: reusable weight-gradient slab workspace of the side stream;
+        attn_seed: int64 [1] device tensor, the step's key of the attention head's element-wise dropout (or None)."""
         self.p = params
         self.g = grads
         self.packed = packed
         self.training = training
         self.drop_mask = drop_mask
+        self.attn_seed = attn_seed
         self.bstat = bstat
         self.stream = stream
         self.sync = sync
@@ -221,12 +223,12 @@ class Engine:
     def _sync(self, bname, direction):
         return self.sync.args(self.pass_id, bname, direction) if self.sync is not None else None
 
-    def rec_backward(self, rec, dz, mask, post_scale=None, g_out=None, g_accumulate=False):
+    def rec_backward(self, rec, dz, mask, post_scale=None, g_out=None, g_accumulate=False, dropout=None):
         """Backward of BN(conv(x)) given the gradient w.r.t. the BN output (dz, optionally ReLU-masked by `mask`)."""
         dy = raw.bn_bwd(dz, mask, post_scale, rec.y, rec.mean, rec.invstd, self.p[rec.bname + ".weight"],
                         self.g[rec.bname + ".weight"], self.g[rec.bname + ".bias"], g_out=g_out,
                         g_accumulate=g_accumulate, sync=self._sync(rec.bname, 1),
-                        cells=self.bncells[rec.bname][1] if self.bncells is not None else None)
+                        cells=self.bncells[rec.bname][1] if self.bncells is not None else None, dropout=dropout)
         x = rec.x
         self.wgrad(x.t, dy, self.g[rec.cname + ".weight"], rec.cout, rec.ksize, rec.stride, rec.dil)
         # a conv bias in front of a training-mode BN has an exactly zero gradient (BN removes the mean): left at 0
@@ -238,7 +240,8 @@ class Engine:
                 raw.conv2d_dgrad(dy, w_d, tuple(x.t.shape), rec.ksize, rec.stride, addend=x.grad, out=x.grad,
                                  dilation=rec.dil)
 
-    def bn_act(self, rec, relu=True, residual=None, out=None, post_scale=None):
+    def bn_act(self, rec, relu=True, residual=None, out=None, post_scale=None, dropout=None):
+        """dropout: (int64 [1] seed tensor, pass index) of an element-wise Dropout(0.5) after the ReLU, or None."""
         if rec.pending is not None:       # deferred finalisation: this pass turns the cells into the layer's parameters
             bn = rec.bname
             kw = dict(batch_out=self.bstat[bn]) if self.bstat is not None else dict(
@@ -246,11 +249,11 @@ class Engine:
                 nbt=self.p[bn + ".num_batches_tracked"])
             z = raw.bn_apply_cells(rec.y, rec.pending, rec.par, self.p[bn + ".weight"], self.p[bn + ".bias"], BN_EPS,
                                    BN_MOMENTUM, residual.t if residual is not None else None, post_scale, relu, out=out,
-                                   **kw)
+                                   dropout=dropout, **kw)
             rec.pending = None
         else:
             z = raw.bn_apply(rec.y, rec.scale, rec.shift, residual.t if residual is not None else None, post_scale,
-                             relu, out=out)
+                             relu, out=out, dropout=dropout)
         za = Act(z)
 
         def bwd():
@@ -264,13 +267,13 @@ class Engine:
                 else:
                     g_acc = True
                 g_out = residual.grad
-            self.rec_backward(rec, dz, z if relu else None, post_scale, g_out, g_acc)
+            self.rec_backward(rec, dz, z if relu else None, post_scale, g_out, g_acc, dropout)
             za.grad = None
         self._push(bwd)
         return za
 
     def conv_bn(self, x, cname, bname, ksize, stride=1, relu=True, residual=None, out=None, bias=False,
-                post_scale=None, dilation=1):
+                post_scale=None, dilation=1, dropout=None):
         if not self.training and post_scale is None:
             # evaluation: BatchNorm (running statistics), residual sum and ReLU in the convolution epilogue - one launch
             w_f, _ = self.packed[cname]
@@ -281,7 +284,7 @@ class Engine:
                                       addend=residual.t if residual is not None else None, out=out, dilation=dilation)
             return Act(z)
         rec = self.conv_stats(x, cname, bname, ksize, stride, bias, dilation, defer=True)
-        return self.bn_act(rec, relu, residual, out, post_scale)
+        return self.bn_act(rec, relu, residual, out, post_scale, dropout)
 
     # ------------------------------------------------------------------------------------------ pre-activation networks
     def _add_grad(self, act, g):

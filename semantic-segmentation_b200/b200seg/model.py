@@ -218,12 +218,17 @@ def ocr_block(E, feats_in, ocfg, p="ocr"):
     return cls, aux, ocr_feats
 
 
-def attn_head(E, x, p="scale_attn"):
-    """make_attn_head (network/utils.py:343-367): returns the PRE-sigmoid logit HeadRec ([N,h,w,1] fp32); the sigmoid
-    is applied where the map is consumed (mscale kernels)."""
-    t = E.conv_bn(x, p + ".conv0", p + ".bn0", 3)
-    t = E.conv_bn(t, p + ".conv1", p + ".bn1", 3)
-    return E.conv_head(t, p + ".conv2", bias=False, ld=1)
+def attn_head(E, x, ocfg=A.OCR_DEFAULT, drop_pass=0):
+    """make_attn_head / old_make_attn_head (network/utils.py:343-382) in the variant ocfg selects (A.attn_head_plan):
+    returns the PRE-sigmoid logit HeadRec ([N,h,w,1] fp32); the sigmoid is applied where the map is consumed (mscale
+    kernels). In training, nn.Dropout(0.5) is fused into the last BatchNorm apply pass (and its backward) with keep bits
+    drawn from E.attn_seed; drop_pass gives each scale pass of the step its own bits."""
+    stages, last, drop = A.attn_head_plan(ocfg)
+    t = x
+    for i, (c, b) in enumerate(stages):
+        d = (E.attn_seed, drop_pass) if drop and E.training and i == len(stages) - 1 else None
+        t = E.conv_bn(t, c, b, 3, dropout=d)
+    return E.conv_head(t, last, bias=False, ld=1)
 
 
 def seg_head(E, x, p="seg_head"):
@@ -304,15 +309,16 @@ def deepv3_pass(E, images, wcfg, size_hw, drop_mask):
 
 
 # ----------------------------------------------------------------------------------------------- per-scale pass
-def scale_pass(E, images, size_hw, arch, hcfg, ocfg, drop_mask=None):
+def scale_pass(E, images, size_hw, arch, hcfg, ocfg, drop_mask=None, drop_pass=0):
     """MscaleOCR._fwd (network/ocrnet.py:170-183) up to the quarter-resolution maps (the x4 Upsample is fused into the
     blend/loss kernels). images: fp32 NCHW; size_hw: pass input size (ResizeX folded into image_prep).
     mscale.DeepV3W38: MscaleV3Plus._fwd (network/mscale.py:296-328) up to the half-resolution maps; drop_mask: this
     pass' WRN-38 Dropout2d multipliers (deepv3_pass). basic.HRNet_ASP / mscale.HRNet_ASP: the ASPP models over the
-    HRNet trunk, up to their quarter-resolution maps."""
+    HRNet trunk, up to their quarter-resolution maps. drop_pass: this pass' index in the attention head's dropout key
+    (attn_head)."""
     if arch == "mscale.DeepV3W38":     # both heads read the decoder concat
         cls, cat = deepv3_pass(E, images, hcfg, size_hw, drop_mask)
-        return dict(cls=cls, aux=None, attn=attn_head(E, cat))
+        return dict(cls=cls, aux=None, attn=attn_head(E, cat, ocfg, drop_pass))
     x16 = Act(raw.image_prep(images, size_hw[0], size_hw[1]), needs_grad=False)
     feats = hrnet_forward(E, x16, hcfg)
     if A.has_hrnet_aspp(arch):
@@ -321,13 +327,13 @@ def scale_pass(E, images, size_hw, arch, hcfg, ocfg, drop_mask=None):
         # attention head on the same 256-channel map
         x = E.conv_sum(aspp(E, feats, ocfg["aspp_bot_ch"]), "bot_aspp", 1)
         cls = seg_head(E, x, "final")
-        return dict(cls=cls, aux=None, attn=attn_head(E, x) if arch == "mscale.HRNet_ASP" else None)
+        return dict(cls=cls, aux=None, attn=attn_head(E, x, ocfg, drop_pass) if arch == "mscale.HRNet_ASP" else None)
     if arch == "basic.HRNet":
         return dict(cls=seg_head(E, feats), aux=None, attn=None)
     if arch == "mscale.HRNet":      # MscaleBasic._fwd (network/mscale.py:463-470): both heads read the trunk features
-        return dict(cls=seg_head(E, feats, "cls_head"), aux=None, attn=attn_head(E, feats))
+        return dict(cls=seg_head(E, feats, "cls_head"), aux=None, attn=attn_head(E, feats, ocfg, drop_pass))
     cls, aux, mid_feats = ocr_block(E, feats, ocfg)
-    attn = attn_head(E, mid_feats) if arch == "ocrnet.HRNet_Mscale" else None
+    attn = attn_head(E, mid_feats, ocfg, drop_pass) if arch == "ocrnet.HRNet_Mscale" else None
     return dict(cls=cls, aux=aux, attn=attn)
 
 
@@ -369,13 +375,13 @@ def train_loss(E, images, gts, arch, hcfg, ocfg, lo_scale=0.5, ocr_alpha=0.4, su
         if par:
             E_lo.stream.wait_stream(main)
             with torch.cuda.stream(E_lo.stream):
-                lo = scale_pass(E_lo, images, (hm, wm), arch, hcfg, ocfg, lo_mask)
+                lo = scale_pass(E_lo, images, (hm, wm), arch, hcfg, ocfg, lo_mask, drop_pass=0)
         else:
-            lo = scale_pass(E, images, (hm, wm), arch, hcfg, ocfg, lo_mask)
+            lo = scale_pass(E, images, (hm, wm), arch, hcfg, ocfg, lo_mask, drop_pass=0)
     if A.has_wrn38_trunk(arch) and not two_scale:
         hi = dict(cls=deepv3_pass(E, images, hcfg, (H, W), hi_mask)[0], aux=None, attn=None)
     else:
-        hi = scale_pass(E, images, (H, W), arch, hcfg, ocfg, hi_mask)
+        hi = scale_pass(E, images, (H, W), arch, hcfg, ocfg, hi_mask, drop_pass=1)
     if par:
         main.wait_stream(E_lo.stream)
     nheads = 2 if A.has_ocr(arch) else 1

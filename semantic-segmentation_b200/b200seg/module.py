@@ -122,9 +122,8 @@ class B200SegModule(nn.Module):
         self.hcfg = hcfg or (A.WRN38 if self.is_deepv3 else A.HRNET_W48)
         self._stem = "backbone.mod1.conv1.weight" if self.is_deepv3 else "backbone.conv1.weight"
         self.wrn_dropout_scale = 1.0     # tests set 0.0 for a dropout-free step
-        self.ocfg = dict(ocfg or A.OCR_DEFAULT)
+        self.ocfg = dict(A.OCR_DEFAULT, **(ocfg or {}))
         self.ocfg["num_classes"] = num_classes
-        self.ocfg.setdefault("aspp_bot_ch", A.OCR_DEFAULT["aspp_bot_ch"])
         if num_classes != 19:
             raise NotImplementedError("the loss / soft-region kernels are instantiated for the 19 Cityscapes classes")
         red = self.ocfg["aspp_bot_ch"]
@@ -133,6 +132,15 @@ class B200SegModule(nn.Module):
             # 16-channel groups (csrc/wgrad_igemm.cu)
             raise NotImplementedError("cfg.MODEL.ASPP_BOT_CH must be a positive multiple of 16 on the sm_90a "
                                       "convolutions; got %d" % red)
+        if arch == "mscale.DeepV3W38" and self.ocfg["mscale_oldarch"]:
+            raise NotImplementedError("cfg.MODEL.MSCALE_OLDARCH (--mscale_old_arch) is not provided on "
+                                      "mscale.DeepV3W38: of the attention-head options only --mscale_no3x3 is")
+        if arch == "mscale.DeepV3W38" and A.attn_head_plan(self.ocfg)[2]:
+            # MscaleV3Plus builds the WRN-38 trunk first, and WiderResNetA2.__init__ rebinds torch.nn.Dropout to
+            # Dropout2d for the whole process (network/wider_resnet.py:302): the head's `drop` is a channel dropout there
+            raise NotImplementedError("cfg.MODEL.MSCALE_DROPOUT on mscale.DeepV3W38 is not covered: the reference's "
+                                      "head dropout is Dropout2d(0.5) on that arch, only the element-wise "
+                                      "Dropout(0.5) of the HRNet archs is on the sm_90a path")
         self.lo_scale, self.ocr_alpha, self.sup_wt, self.ignore_index = lo_scale, ocr_alpha, supervised_mscale_wt, ignore_index
         self.n_scales = n_scales
         self.use_cuda_graph = use_cuda_graph
@@ -167,7 +175,9 @@ class B200SegModule(nn.Module):
         nn.Conv2d default (kaiming_uniform(a=sqrt(5)), bias U(+-1/sqrt(fan_in))) as in network/ocrnet.py:46-83.
         mscale.DeepV3W38 initialises only `final` (plus bot_* and scale_attn with init_decoder) with kaiming_normal_;
         ASPP and the rest keep the nn.Conv2d default (network/mscale.py:272-278). basic.HRNet_ASP initialises `final`,
-        `bot_aspp` and `aspp` (network/basic.py:82), mscale.HRNet_ASP only `final` (network/mscale.py:494)."""
+        `bot_aspp` and `aspp` (network/basic.py:82), mscale.HRNet_ASP only `final` (network/mscale.py:494).
+        The old attention head (cfg.MODEL.MSCALE_OLDARCH) is built by old_make_attn_head, whose init_attn zeroes its
+        convolution weights (network/utils.py:332-341,381)."""
         if self.arch == "mscale.DeepV3W38":
             kaiming_normal = ("final", "bot_fine", "bot_aspp", "scale_attn") if self.init_decoder else ("final",)
         elif self.arch == "mscale.HRNet_ASP":
@@ -186,6 +196,8 @@ class B200SegModule(nn.Module):
                 if parts[0] in kaiming_normal:
                     # initialize_weights = kaiming_normal_ (network/deepv3.py:66-69, network/mynn.py:27-39)
                     nn.init.kaiming_normal_(w)
+                elif parts[0] == "scale_attn" and self.ocfg["mscale_oldarch"]:
+                    w.zero_()           # init_attn
                 elif self.is_deepv3:
                     # WRN-38 trunk and the layers initialize_weights leaves alone: nn.Conv2d default
                     nn.init.kaiming_uniform_(w, a=math.sqrt(5))
@@ -386,11 +398,11 @@ class B200SegModule(nn.Module):
         return evt
 
     # ------------------------------------------------------------------------------------------ training step
-    def _step_eager(self, images, gts, drop_mask):
+    def _step_eager(self, images, gts, drop_mask, attn_seed=None):
         from . import _lib
         launches0 = _lib.KERNEL_LAUNCHES
         try:
-            return self._step_body(images, gts, drop_mask)
+            return self._step_body(images, gts, drop_mask, attn_seed)
         finally:
             raw.KEEP = None
             self.kernels_per_step = _lib.KERNEL_LAUNCHES - launches0   # same count when the captured graph replays
@@ -409,7 +421,7 @@ class B200SegModule(nn.Module):
             self._graphs = {}
         return self._sync
 
-    def _step_body(self, images, gts, drop_mask):
+    def _step_body(self, images, gts, drop_mask, attn_seed=None):
         if getattr(self, "_side_stream", None) is None:
             self._side_stream = torch.cuda.Stream()
         sync = self._sync
@@ -444,14 +456,14 @@ class B200SegModule(nn.Module):
             E_lo = Engine(tensors, grads_lo, self._packed, True, drop_mask, side_stream=self._side_stream_lo,
                           bstat=self._bstat_views[0], stream=self._lo_stream, sync=sync, pass_id=0,
                           branch_streams=self._bstreams["lo"], ws_holder=self._ws_holders["lo"],
-                          bncells=self._bncells[0] if use_cells else None)
+                          bncells=self._bncells[0] if use_cells else None, attn_seed=attn_seed)
         two_pass = A.is_two_scale(self.arch)
         if sync is not None and two_pass and not par:
             raise RuntimeError("SyncBN needs parallel_scales=True for the two-scale step (one engine per pass)")
         E = Engine(tensors, grads, self._packed, True, drop_mask, side_stream=self._side_stream,
                    bstat=self._bstat_views[1] if par else None, sync=sync, pass_id=1 if two_pass else 0,
                    branch_streams=self._bstreams["hi"], ws_holder=self._ws_holders["hi"],
-                   bncells=self._bncells[1] if use_cells else None)
+                   bncells=self._bncells[1] if use_cells else None, attn_seed=attn_seed)
         loss = M.train_loss(E, images, gts, self.arch, self.hcfg, self.ocfg, self.lo_scale, self.ocr_alpha, self.sup_wt,
                             self.ignore_index, E_lo=E_lo, loss_kind=self.loss_kind, img_wt=self.img_wt,
                             ocr_aux_rmi=self.ocr_aux_rmi)
@@ -488,6 +500,14 @@ class B200SegModule(nn.Module):
         keep = torch.bernoulli(torch.full((n, c), 1.0 - p, dtype=F32, device=device))
         return keep / (1.0 - p)
 
+    def _attn_seed(self, device):
+        """Key of the attention head's element-wise Dropout(0.5) (cfg.MODEL.MSCALE_DROPOUT) for one step: an int64 drawn
+        on the device from torch's CUDA generator (no host synchronisation); the kernels derive every keep bit from it
+        (csrc/dropout.cuh), so no mask is stored. None when the head has no dropout."""
+        if not (A.is_two_scale(self.arch) and A.attn_head_plan(self.ocfg)[2]):
+            return None
+        return torch.randint(-2 ** 63, 2 ** 63 - 1, (1,), dtype=torch.int64, device=device)
+
     def _train_forward(self, images, gts):
         self._ensure_device_state()
         self._sync_context()
@@ -495,25 +515,29 @@ class B200SegModule(nn.Module):
         gts = gts.contiguous().long()
         key = (tuple(images.shape), str(images.device))
         mask = self._drop_mask(images.shape[0], images.device)
+        seed = self._attn_seed(images.device)
+        self.last_attn_seed = seed
         if not self.use_cuda_graph:
-            return self._step_eager(images, gts, mask)
+            return self._step_eager(images, gts, mask, seed)
         st = self._graphs.get(key)
         if st is None:
-            st = dict(images=images.clone(), gts=gts.clone(), mask=None if mask is None else mask.clone(), calls=0,
-                      graph=None, loss=None)
+            st = dict(images=images.clone(), gts=gts.clone(), mask=None if mask is None else mask.clone(),
+                      seed=None if seed is None else seed.clone(), calls=0, graph=None, loss=None)
             self._graphs[key] = st
         st["images"].copy_(images)
         st["gts"].copy_(gts)
         if mask is not None:
             st["mask"].copy_(mask)
+        if seed is not None:
+            st["seed"].copy_(seed)
         st["calls"] += 1
         if st["graph"] is None:
             if st["calls"] < 2:      # first call: eager warm-up (sets kernel attributes, fills the allocator pools)
-                return self._step_eager(st["images"], st["gts"], st["mask"])
+                return self._step_eager(st["images"], st["gts"], st["mask"], st["seed"])
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
-                st["loss"] = self._step_eager(st["images"], st["gts"], st["mask"])
+                st["loss"] = self._step_eager(st["images"], st["gts"], st["mask"], st["seed"])
             st["graph"] = g
         st["graph"].replay()
         return st["loss"]

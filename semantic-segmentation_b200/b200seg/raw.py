@@ -203,8 +203,17 @@ def conv2d_fwd_cells(x, w_ohwi, bias, stride, cells, out=None, dilation=1):
     return out
 
 
+def _drop_args(dropout):
+    """(int64 [1] seed tensor, pass index) or None -> the (drop_seed, drop_pass) arguments of the BatchNorm passes."""
+    if dropout is None:
+        return None, 0
+    seed, pass_idx = dropout
+    assert seed.is_cuda and seed.dtype == torch.int64 and seed.numel() == 1
+    return ptr(seed), int(pass_idx)
+
+
 def bn_apply_cells(y, cells, par, gamma, beta, eps, momentum, res=None, post_scale=None, relu=True, out=None,
-                   batch_out=None, running_mean=None, running_var=None, nbt=None):
+                   batch_out=None, running_mean=None, running_var=None, nbt=None, dropout=None):
     """bn_apply as the consumer of conv2d_fwd_cells: finalises the statistics in its prologue and fills par (fp32
     [4, c] = scale, shift, mean, invstd) and the batch / running statistics."""
     n, h, w, c = y.shape
@@ -213,7 +222,7 @@ def bn_apply_cells(y, cells, par, gamma, beta, eps, momentum, res=None, post_sca
     f = _cells_fold(cells, par, gamma, beta, eps, momentum, n * h * w, c, batch_out, running_mean, running_var, nbt)
     check(lib().b200seg_bn_apply_cells(ptr(y), _ld(y), ctypes.byref(f), ptr(res), _ld(res) if res is not None else 0,
                                        ptr(post_scale), int(relu), ptr(out), _ld(out), n * h * w, h * w, c,
-                                       stream_ptr()), "bn_apply_cells")
+                                       *_drop_args(dropout), stream_ptr()), "bn_apply_cells")
     return out
 
 
@@ -324,21 +333,25 @@ def accum_f32(dst, src):
     check(lib().b200seg_accum_f32(ptr(dst), ptr(src), dst.numel(), stream_ptr()), "accum_f32")
 
 
-def bn_apply(y, scale, shift, res=None, post_scale=None, relu=True, out=None):
+def bn_apply(y, scale, shift, res=None, post_scale=None, relu=True, out=None, dropout=None):
+    """dropout: (int64 [1] seed tensor, pass index): element-wise Dropout(0.5) after the ReLU (include/b200seg.h)."""
     n, h, w, c = y.shape
     if out is None:
         out = _new((n, h, w, c), dtype=BF16, device=y.device)
     check(lib().b200seg_bn_apply(ptr(y), _ld(y), ptr(scale), ptr(shift), ptr(res), _ld(res) if res is not None else 0,
-                                 ptr(post_scale), int(relu), ptr(out), _ld(out), n * h * w, h * w, c, stream_ptr()),
+                                 ptr(post_scale), int(relu), ptr(out), _ld(out), n * h * w, h * w, c,
+                                 *_drop_args(dropout), stream_ptr()),
           "bn_apply")
     return out
 
 
 def bn_bwd(dz, mask, post_scale, y, mean, invstd, gamma, dgamma, dbeta, g_out=None, g_accumulate=False, dy_out=None,
-           sync=None, cells=None):
+           sync=None, cells=None, dropout=None):
     """Returns dy (gradient w.r.t. the BN input). dgamma/dbeta (fp32 views) are accumulated into. cells (fp64 [2*c],
-    zero at the start of the step): deferred finalisation inside the gradient pass (two launches, per-GPU statistics)."""
+    zero at the start of the step): deferred finalisation inside the gradient pass (two launches, per-GPU statistics).
+    dropout: the (seed, pass) of the forward apply pass, whose keep bits are regenerated and applied to dz."""
     n, h, w, c = y.shape
+    drop = _drop_args(dropout)
     npix = n * h * w
     L = lib()
     if cells is not None and sync is None:
@@ -346,22 +359,32 @@ def bn_bwd(dz, mask, post_scale, y, mean, invstd, gamma, dgamma, dbeta, g_out=No
         check(L.b200seg_bn_bwd_cells(ptr(dz), _ld(dz), ptr(mask), _ld(mask) if mask is not None else 0, ptr(post_scale),
                                      ptr(y), _ld(y), ptr(mean), ptr(invstd), ptr(gamma), ptr(dgamma), ptr(dbeta),
                                      ptr(cells), ptr(dy), _ld(dy), ptr(g_out), _ld(g_out) if g_out is not None else 0,
-                                     int(g_accumulate), npix, h * w, c, stream_ptr()), "bn_bwd_cells", launches=2)
+                                     int(g_accumulate), npix, h * w, c, *drop, stream_ptr()), "bn_bwd_cells",
+              launches=2)
         return dy
     cc = _new((2, c), dtype=F32, device=y.device)
     grid = L.b200seg_bn_bwd_grid(npix, c)
     partials = _new((grid, 2, c), dtype=F32, device=y.device)
     check(L.b200seg_bn_bwd_reduce(ptr(dz), _ld(dz), ptr(mask), _ld(mask) if mask is not None else 0,
                                   ptr(post_scale), ptr(y), _ld(y), ptr(mean), ptr(invstd), npix, h * w, c,
-                                  ptr(partials), stream_ptr()), "bn_bwd_reduce")
+                                  ptr(partials), *drop, stream_ptr()), "bn_bwd_reduce")
     check(L.b200seg_bn_bwd_finalize(ptr(partials), grid, c, float(npix), ptr(dgamma), ptr(dbeta), ptr(cc[0]),
                                     ptr(cc[1]), _sync_ref(sync), stream_ptr()), "bn_bwd_finalize")
     dy = dy_out if dy_out is not None else _new((n, h, w, c), dtype=BF16, device=y.device)
     check(L.b200seg_bn_bwd_apply(ptr(dz), _ld(dz), ptr(mask), _ld(mask) if mask is not None else 0, ptr(post_scale),
                                  ptr(y), _ld(y), ptr(mean), ptr(invstd), ptr(gamma), ptr(cc[0]), ptr(cc[1]), ptr(dy),
                                  _ld(dy), ptr(g_out), _ld(g_out) if g_out is not None else 0, int(g_accumulate), npix,
-                                 h * w, c, stream_ptr()), "bn_bwd_apply")
+                                 h * w, c, *drop, stream_ptr()), "bn_bwd_apply")
     return dy
+
+
+def dropout_keep_mask(seed, pass_idx, npix, c):
+    """Test library: the uint8 [npix * c] keep mask the BatchNorm passes apply for (seed, pass_idx)."""
+    from ._lib import test_lib
+    mask = _new(npix * c, dtype=torch.uint8, device=seed.device)
+    check(test_lib().b200seg_dropout_keep_mask(*_drop_args((seed, pass_idx)), npix, c, ptr(mask), stream_ptr()),
+          "dropout_keep_mask")
+    return mask
 
 
 def masked_accum(src, mask, dst, accumulate):

@@ -3,7 +3,8 @@
 // running estimate). All kernels are HBM-bound streaming passes over NHWC bf16 with 16-byte vector accesses.
 //
 //   forward : conv epilogue partials -> bn_finalize (scale/shift/mean/invstd + running stats) -> bn_apply
-//             z = relu?( (y*scale + shift [+ residual]) ) [* post_scale[n][c]]          (Dropout2d folded in post_scale)
+//             z = relu?( (y*scale + shift [+ residual]) ) [* post_scale[n][c]] [* 2 keep]  (Dropout2d folded in
+//             post_scale; element-wise Dropout(0.5) keep bits regenerated from the step's seed, dropout.cuh)
 //   backward: bn_bwd_reduce (sum g, sum g*xhat per channel; g = dz * (mask>0)) -> bn_bwd_finalize (dgamma, dbeta, c1, c2)
 //             -> bn_bwd_apply  dy = gamma*invstd*(g - c1 - xhat*c2)  [and g written out for the residual branch]
 #include "ptx.cuh"
@@ -11,6 +12,7 @@
 #include "../../include/b200seg.h"
 #include "vec.cuh"
 #include "conv_common.h"
+#include "dropout.cuh"
 #include <cstring>
 
 namespace b200seg {
@@ -293,13 +295,16 @@ struct BnLazy {
   long long* nbt;
 };
 
+// kDrop: the element-wise dropout is compiled in only where it is used, so the passes without it keep their code
+template <bool kDrop>
 __global__ void __launch_bounds__(256)
 bn_apply_kernel(const __nv_bfloat16* __restrict__ y, int y_ld, float* __restrict__ scale,
                 float* __restrict__ shift, const __nv_bfloat16* __restrict__ res, int res_ld,
                 const float* __restrict__ post_scale, int relu, __nv_bfloat16* __restrict__ z, int z_ld,
-                long long npix, int hw, int C, const BnLazy lazy) {
+                long long npix, int hw, int C, const BnLazy lazy, const DropKey drop) {
   pdl_sync();
   extern __shared__ float s_par[];   // [2][C]
+  const unsigned long long dseed = kDrop ? *drop.seed : 0ull;
   if (lazy.cells != nullptr) {
     for (int c = threadIdx.x; c < C; c += blockDim.x) {
       const double s1 = lazy.cells[c], s2 = lazy.cells[lazy.cpad + c];
@@ -361,6 +366,7 @@ bn_apply_kernel(const __nv_bfloat16* __restrict__ y, int y_ld, float* __restrict
 #pragma unroll
         for (int j = 0; j < 8; ++j) v[j] *= ps[j];
       }
+      if (kDrop) dropout_apply8(v, dseed, drop.pass, pix[u] * C + c0[u]);
       store8(z + pix[u] * z_ld + c0[u], v);
     }
   }
@@ -371,12 +377,14 @@ bn_apply_kernel(const __nv_bfloat16* __restrict__ y, int y_ld, float* __restrict
 // Thread (r, cg): r-th pixel row of the block, 8-channel group cg. blockDim.x = groups * rows. The block's sums go to
 // `cells` ([2][C] fp64, added; bn_bwd_apply folds them) or, when cells == nullptr, to its row of `partials`
 // (bn_bwd_finalize folds them).
+template <bool kDrop>
 __global__ void __launch_bounds__(256)
 bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ dz, int dz_ld, const __nv_bfloat16* __restrict__ mask,
                      int mask_ld, const float* __restrict__ post_scale, const __nv_bfloat16* __restrict__ y, int y_ld,
                      const float* __restrict__ mean, const float* __restrict__ invstd, long long npix, int hw, int C,
-                     int rows, float* __restrict__ partials, double* __restrict__ cells) {
+                     int rows, float* __restrict__ partials, double* __restrict__ cells, const DropKey drop) {
   pdl_sync();
+  const unsigned long long dseed = kDrop ? *drop.seed : 0ull;
   extern __shared__ float s_red[];   // [rows][groups][16]
   const int groups = C >> 3;
   const int cg = threadIdx.x % groups, r = threadIdx.x / groups;
@@ -409,6 +417,7 @@ bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ dz, int dz_ld, const __nv
 #pragma unroll
           for (int j = 0; j < 8; ++j) g[j] *= ps[j];
         }
+        if (kDrop) dropout_apply8(g, dseed, drop.pass, pix * C + c0);
         if (mask) {
           float mk[8];
           unpack8(mq[u], mk);
@@ -484,6 +493,7 @@ bn_bwd_sync_finish_kernel(int C, float count, float* __restrict__ c1, float* __r
   }
 }
 
+template <bool kDrop>
 __global__ void __launch_bounds__(256)
 bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ dz, int dz_ld, const __nv_bfloat16* __restrict__ mask,
                     int mask_ld, const float* __restrict__ post_scale, const __nv_bfloat16* __restrict__ y, int y_ld,
@@ -491,8 +501,9 @@ bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ dz, int dz_ld, const __nv_
                     const float* __restrict__ c1, const float* __restrict__ c2, __nv_bfloat16* __restrict__ dy, int dy_ld,
                     __nv_bfloat16* __restrict__ g_out, int g_ld, int g_accumulate, long long npix, int hw, int C,
                     const double* __restrict__ cells, float count, float* __restrict__ dgamma,
-                    float* __restrict__ dbeta) {
+                    float* __restrict__ dbeta, const DropKey drop) {
   pdl_sync();
+  const unsigned long long dseed = kDrop ? *drop.seed : 0ull;
   extern __shared__ float s_par[];   // [5][C]: mean, invstd, gamma*invstd, c1, c2
   for (int i = threadIdx.x; i < C; i += blockDim.x) {
     s_par[i] = mean[i];
@@ -545,6 +556,7 @@ bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ dz, int dz_ld, const __nv_
 #pragma unroll
         for (int j = 0; j < 8; ++j) g[j] *= ps[j];
       }
+      if (kDrop) dropout_apply8(g, dseed, drop.pass, pix * C + c0);
       if (mask) {
         float mk[8];
         unpack8(mq[u], mk);
@@ -632,6 +644,13 @@ static int make_sync(const b200seg_bn_sync* s, SyncArgs* out) {
   return 0;
 }
 
+static inline DropKey drop_key(const uint64_t* seed, int32_t pass) {
+  DropKey d;
+  d.seed = (const unsigned long long*)seed;
+  d.pass = pass;
+  return d;
+}
+
 #define CHECK_LAUNCH()                      \
   do {                                      \
     cudaError_t e_ = cudaGetLastError();    \
@@ -677,19 +696,23 @@ extern "C" int b200seg_accum_f32(float* dst, const float* src, int64_t n, void* 
 
 extern "C" int b200seg_bn_apply(const void* y, int32_t y_ld, const float* scale, const float* shift, const void* res,
                                 int32_t res_ld, const float* post_scale, int32_t relu, void* z, int32_t z_ld,
-                                int64_t npix, int32_t hw, int32_t c, void* stream) {
+                                int64_t npix, int32_t hw, int32_t c, const uint64_t* drop_seed, int32_t drop_pass,
+                                void* stream) {
   if (!y || !z || !scale || !shift || c % 8 || y_ld % 8 || z_ld % 8 || (res && res_ld % 8)) return B200SEG_E_BADARG;
   BnLazy lazy;
   memset(&lazy, 0, sizeof(lazy));
-  launch_k(bn_apply_kernel, dim3(ew_grid(npix * (c / 8))), dim3(256), 2 * c * sizeof(float), (cudaStream_t)stream,
-           (const __nv_bfloat16*)y, y_ld, const_cast<float*>(scale), const_cast<float*>(shift),
-           (const __nv_bfloat16*)res, res_ld, post_scale, relu, (__nv_bfloat16*)z, z_ld, npix, hw, c, lazy);
+  launch_k(drop_seed ? bn_apply_kernel<true> : bn_apply_kernel<false>, dim3(ew_grid(npix * (c / 8))), dim3(256),
+           2 * c * sizeof(float), (cudaStream_t)stream, (const __nv_bfloat16*)y, y_ld, const_cast<float*>(scale),
+           const_cast<float*>(shift),
+           (const __nv_bfloat16*)res, res_ld, post_scale, relu, (__nv_bfloat16*)z, z_ld, npix, hw, c, lazy,
+           drop_key(drop_seed, drop_pass));
   CHECK_LAUNCH();
 }
 
 extern "C" int b200seg_bn_apply_cells(const void* y, int32_t y_ld, const b200seg_bn_fold* f, const void* res,
                                       int32_t res_ld, const float* post_scale, int32_t relu, void* z, int32_t z_ld,
-                                      int64_t npix, int32_t hw, int32_t c, void* stream) {
+                                      int64_t npix, int32_t hw, int32_t c, const uint64_t* drop_seed,
+                                      int32_t drop_pass, void* stream) {
   if (!y || !z || !f || c % 8 || y_ld % 8 || z_ld % 8 || (res && res_ld % 8)) return B200SEG_E_BADARG;
   if (!f->accum || !f->scale || !f->shift || !f->mean || !f->invstd || f->c != c || f->count <= 0.f ||
       (reinterpret_cast<uintptr_t>(f->accum) & 7))
@@ -700,9 +723,9 @@ extern "C" int b200seg_bn_apply_cells(const void* y, int32_t y_ld, const b200seg
   lazy.gamma = f->gamma; lazy.beta = f->beta; lazy.mean_out = f->mean; lazy.invstd_out = f->invstd;
   lazy.batch_stats_out = f->batch_stats_out; lazy.running_mean = f->running_mean; lazy.running_var = f->running_var;
   lazy.nbt = (long long*)f->num_batches_tracked;
-  launch_k(bn_apply_kernel, dim3(ew_grid(npix * (c / 8))), dim3(256), 2 * c * sizeof(float), (cudaStream_t)stream,
-           (const __nv_bfloat16*)y, y_ld, f->scale, f->shift, (const __nv_bfloat16*)res, res_ld, post_scale, relu,
-           (__nv_bfloat16*)z, z_ld, npix, hw, c, lazy);
+  launch_k(drop_seed ? bn_apply_kernel<true> : bn_apply_kernel<false>, dim3(ew_grid(npix * (c / 8))), dim3(256),
+           2 * c * sizeof(float), (cudaStream_t)stream, (const __nv_bfloat16*)y, y_ld, f->scale, f->shift, (const __nv_bfloat16*)res, res_ld, post_scale, relu,
+           (__nv_bfloat16*)z, z_ld, npix, hw, c, lazy, drop_key(drop_seed, drop_pass));
   CHECK_LAUNCH();
 }
 
@@ -726,25 +749,25 @@ extern "C" int32_t b200seg_bn_bwd_grid(int64_t npix, int32_t c) {
 static int bn_bwd_reduce_launch(const void* dz, int32_t dz_ld, const void* mask, int32_t mask_ld,
                                 const float* post_scale, const void* y, int32_t y_ld, const float* mean,
                                 const float* invstd, int64_t npix, int32_t hw, int32_t c, float* partials,
-                                double* cells, void* stream) {
+                                double* cells, DropKey drop, void* stream) {
   if (!dz || !y || !mean || !invstd || (!partials && !cells) || c % 8 || c > 2048) return B200SEG_E_BADARG;
   int rows, threads;
   reduce_shape(c, &rows, &threads);
   if (threads > 256) return B200SEG_E_BADARG;
   const int grid = b200seg_bn_bwd_grid(npix, c);
   const size_t smem = (size_t)rows * (c / 8) * 16 * sizeof(float);
-  launch_k(bn_bwd_reduce_kernel, dim3(grid), dim3(threads), smem, (cudaStream_t)stream, (const __nv_bfloat16*)dz,
+  launch_k(drop.seed ? bn_bwd_reduce_kernel<true> : bn_bwd_reduce_kernel<false>, dim3(grid), dim3(threads), smem, (cudaStream_t)stream, (const __nv_bfloat16*)dz,
            dz_ld, (const __nv_bfloat16*)mask, mask_ld, post_scale, (const __nv_bfloat16*)y, y_ld, mean, invstd, npix,
-           hw, c, rows, partials, cells);
+           hw, c, rows, partials, cells, drop);
   CHECK_LAUNCH();
 }
 
 extern "C" int b200seg_bn_bwd_reduce(const void* dz, int32_t dz_ld, const void* mask, int32_t mask_ld,
                                      const float* post_scale, const void* y, int32_t y_ld, const float* mean,
                                      const float* invstd, int64_t npix, int32_t hw, int32_t c, float* partials,
-                                     void* stream) {
+                                     const uint64_t* drop_seed, int32_t drop_pass, void* stream) {
   return bn_bwd_reduce_launch(dz, dz_ld, mask, mask_ld, post_scale, y, y_ld, mean, invstd, npix, hw, c, partials,
-                              nullptr, stream);
+                              nullptr, drop_key(drop_seed, drop_pass), stream);
 }
 
 extern "C" int b200seg_bn_bwd_finalize(const float* partials, int32_t grid, int32_t c, float count, float* dgamma,
@@ -766,12 +789,14 @@ extern "C" int b200seg_bn_bwd_apply(const void* dz, int32_t dz_ld, const void* m
                                     const float* post_scale, const void* y, int32_t y_ld, const float* mean,
                                     const float* invstd, const float* gamma, const float* c1, const float* c2, void* dy,
                                     int32_t dy_ld, void* g_out, int32_t g_ld, int32_t g_accumulate, int64_t npix,
-                                    int32_t hw, int32_t c, void* stream) {
+                                    int32_t hw, int32_t c, const uint64_t* drop_seed, int32_t drop_pass,
+                                    void* stream) {
   if (!dz || !y || !dy || !mean || !invstd || !c1 || !c2 || c % 8) return B200SEG_E_BADARG;
-  launch_k(bn_bwd_apply_kernel, dim3(ew_grid(npix * (c / 8))), dim3(256), 5 * c * sizeof(float), (cudaStream_t)stream,
+  launch_k(drop_seed ? bn_bwd_apply_kernel<true> : bn_bwd_apply_kernel<false>, dim3(ew_grid(npix * (c / 8))),
+           dim3(256), 5 * c * sizeof(float), (cudaStream_t)stream,
            (const __nv_bfloat16*)dz, dz_ld, (const __nv_bfloat16*)mask, mask_ld, post_scale, (const __nv_bfloat16*)y,
            y_ld, mean, invstd, gamma, c1, c2, (__nv_bfloat16*)dy, dy_ld, (__nv_bfloat16*)g_out, g_ld, g_accumulate,
-           npix, hw, c, (const double*)nullptr, 0.f, (float*)nullptr, (float*)nullptr);
+           npix, hw, c, (const double*)nullptr, 0.f, (float*)nullptr, (float*)nullptr, drop_key(drop_seed, drop_pass));
   CHECK_LAUNCH();
 }
 
@@ -782,16 +807,20 @@ extern "C" int b200seg_bn_bwd_cells(const void* dz, int32_t dz_ld, const void* m
                                     const float* post_scale, const void* y, int32_t y_ld, const float* mean,
                                     const float* invstd, const float* gamma, float* dgamma, float* dbeta, double* cells,
                                     void* dy, int32_t dy_ld, void* g_out, int32_t g_ld, int32_t g_accumulate,
-                                    int64_t npix, int32_t hw, int32_t c, void* stream) {
+                                    int64_t npix, int32_t hw, int32_t c, const uint64_t* drop_seed, int32_t drop_pass,
+                                    void* stream) {
   if (!dz || !y || !dy || !mean || !invstd || !cells || c % 8 || (reinterpret_cast<uintptr_t>(cells) & 7))
     return B200SEG_E_BADARG;
+  const DropKey drop = drop_key(drop_seed, drop_pass);
   if (int rc = bn_bwd_reduce_launch(dz, dz_ld, mask, mask_ld, post_scale, y, y_ld, mean, invstd, npix, hw, c, nullptr,
-                                    cells, stream))
+                                    cells, drop, stream))
     return rc;
-  launch_k(bn_bwd_apply_kernel, dim3(ew_grid(npix * (c / 8))), dim3(256), 5 * c * sizeof(float), (cudaStream_t)stream,
+  launch_k(drop.seed ? bn_bwd_apply_kernel<true> : bn_bwd_apply_kernel<false>, dim3(ew_grid(npix * (c / 8))),
+           dim3(256), 5 * c * sizeof(float), (cudaStream_t)stream,
            (const __nv_bfloat16*)dz, dz_ld, (const __nv_bfloat16*)mask, mask_ld, post_scale, (const __nv_bfloat16*)y,
            y_ld, mean, invstd, gamma, (const float*)nullptr, (const float*)nullptr, (__nv_bfloat16*)dy, dy_ld,
-           (__nv_bfloat16*)g_out, g_ld, g_accumulate, npix, hw, c, (const double*)cells, (float)npix, dgamma, dbeta);
+           (__nv_bfloat16*)g_out, g_ld, g_accumulate, npix, hw, c, (const double*)cells, (float)npix, dgamma, dbeta,
+           drop);
   CHECK_LAUNCH();
 }
 

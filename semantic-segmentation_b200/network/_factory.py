@@ -32,8 +32,15 @@ def build(arch, num_classes, criterion):
         kw["n_scales"] = cfg.MODEL.N_SCALES
         if cfg.MODEL.ALIGN_CORNERS:
             raise NotImplementedError("align_corners=True is not covered by the B200 resampling kernels")
-        if cfg.MODEL.OCR_ASPP or cfg.MODEL.MSCALE_OLDARCH or not cfg.MODEL.MSCALE_INNER_3x3 or cfg.MODEL.MSCALE_DROPOUT:
-            raise NotImplementedError("only the default OCR / attention-head configuration is on the hot path")
+        if cfg.MODEL.OCR_ASPP:
+            raise NotImplementedError("cfg.MODEL.OCR_ASPP (--ocr_aspp) is not covered: the reference itself raises "
+                                      "NameError: name 'get_aspp' is not defined for it (network/ocr_utils.py never "
+                                      "imports get_aspp)")
+        # the attention-head ablations (--mscale_no3x3 / --mscale_dropout / --mscale_old_arch, config.py:318-325),
+        # read by make_attn_head; archs without an attention head ignore them like the reference does
+        ocfg["mscale_inner_3x3"] = bool(cfg.MODEL.MSCALE_INNER_3x3)
+        ocfg["mscale_dropout"] = bool(cfg.MODEL.MSCALE_DROPOUT)
+        ocfg["mscale_oldarch"] = bool(cfg.MODEL.MSCALE_OLDARCH)
         kw["ocr_aux_rmi"] = bool(cfg.LOSS.OCR_AUX_RMI)
         # cfg.MODEL.BNFUNC (config.py:216-225: apex.parallel.SyncBatchNorm under --syncbn --apex, else BatchNorm2d)
         # decides whether BatchNorm statistics span the data-parallel group

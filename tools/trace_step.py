@@ -88,6 +88,9 @@ def main():
                     help="trace the training default with per-GPU statistics: deferred BatchNorm finalisation inside "
                          "the consuming apply passes; without the flag: the program with separate bn_finalize / "
                          "bn_bwd_finalize launches (SyncBN)")
+    ap.add_argument("--attn-head", default="default", choices=["default", "no3x3", "dropout", "oldarch", "no3x3_dropout"],
+                    help="attention-head ablation of the multi-scale archs (--mscale_no3x3 / --mscale_dropout / "
+                         "--mscale_old_arch of the reference's train.py)")
     args = ap.parse_args()
     if __debug__:
         sys.exit("run with python -O (the wrappers assert is_cuda)")
@@ -99,7 +102,11 @@ def main():
     raw.stream_ptr = lambda: 0
 
     from b200seg.module import B200SegModule
-    net = B200SegModule(args.arch, 19)
+    from b200seg import arch as A
+    flags = dict(no3x3=dict(mscale_inner_3x3=False), dropout=dict(mscale_dropout=True),
+                 oldarch=dict(mscale_oldarch=True),
+                 no3x3_dropout=dict(mscale_inner_3x3=False, mscale_dropout=True)).get(args.attn_head, {})
+    net = B200SegModule(args.arch, 19, ocfg=dict(A.OCR_DEFAULT, **flags))
     dev = torch.device("meta")
     tensors = {k: torch.empty(v.shape, dtype=v.dtype, device=dev) for k, v in net._tensors().items()}
     packed, grads = {}, {}
@@ -114,7 +121,6 @@ def main():
             grads[n] = torch.empty(p.shape, dtype=torch.float32, device=dev)
     images = torch.empty((1, 3, args.height, args.width), dtype=torch.float32, device=dev)
     gts = torch.empty((1, args.height, args.width), dtype=torch.long, device=dev)
-    from b200seg import arch as A
     if A.has_wrn38_trunk(args.arch):
         n_sets = 2 if A.is_two_scale(args.arch) else 1        # one Dropout2d mask set per scale pass
         mask = torch.empty((n_sets * sum(c for _b, c, _p in A.wrn_drop_layout(net.hcfg)),), dtype=torch.float32,
@@ -126,7 +132,8 @@ def main():
         bncells = {n[: -len(".running_mean")]: (torch.empty(2 * ((v.shape[0] + 15) // 16 * 16), dtype=torch.float64, device=dev),
                                                 torch.empty(2 * v.shape[0], dtype=torch.float64, device=dev))
                    for n, v in tensors.items() if n.endswith(".running_mean")}
-    E = EN.Engine(tensors, grads, packed, True, mask, bncells=bncells)
+    E = EN.Engine(tensors, grads, packed, True, mask, bncells=bncells,
+                  attn_seed=torch.empty((1,), dtype=torch.int64, device=dev))
     M.train_loss(E, images, gts, args.arch, net.hcfg, net.ocfg)
     n_fwd = len(EVENTS)
     M.run_backward(E)
