@@ -54,10 +54,14 @@ typedef struct b200seg_conv_desc {
                               network/wider_resnet.py:322-330, network/utils.py:176-192) */
 } b200seg_conv_desc;
 
-/* Host-only introspection of the launch plan (tests, tuning): which = 0 forward, 1 stride-1 data gradient.
+/* Host-only introspection of the launch plan (tests, tuning): which = 0 forward, 1 stride-1 data gradient; the kernel
+ * reported is the one the launch entry points run for the same descriptor (dilation, out_fp32 and emit_stats count).
  * out[12] = {kernel (1 = halo-tile 3x3, 0 = per-tap implicit GEMM), Cout tile, Cout tiles, grid, dynamic shared memory
  * bytes, ring depth, CTAs per SM, accumulator registers per thread, resident weights, weight slots, channel chunk per
- * pipeline stage (16/32/64), tiles (pixel tiles x Cout tiles)}. Returns 0 or a negative error. */
+ * pipeline stage (16/32/64), tiles (pixel tiles x Cout tiles)}. With which | B200SEG_PLAN_WINDOW, out holds 13 entries
+ * and out[12] is the statistics window (1 = with emit_stats every CTA keeps only its own Cout tile's statistics columns
+ * and writes zeros in the others; always 0 for the halo kernel). Returns 0 or a negative error. */
+#define B200SEG_PLAN_WINDOW 0x100
 int b200seg_conv2d_plan_info(const b200seg_conv_desc* d, int32_t which, int32_t* out);
 
 /* Host-only introspection of the weight-gradient plan (b200seg_conv2d_wgrad): out[10] = {N tile width in input channels

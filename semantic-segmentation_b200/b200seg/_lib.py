@@ -10,6 +10,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # B200SEG_LIB_VARIANT=<tag> loads lib/libb200seg_<tag>.so (A/B of compile-time switches, csrc/Makefile); default: the product
 _VARIANT = os.environ.get("B200SEG_LIB_VARIANT", "")
 LIB_PATH = os.path.join(_HERE, "lib", "libb200seg%s.so" % (("_" + _VARIANT) if _VARIANT else ""))
+# b200seg_conv2d_plan_info: which | PLAN_WINDOW asks for the 13-entry form with the statistics window in out[12]
+PLAN_WINDOW = 0x100
 
 c_int32 = ctypes.c_int32
 c_int64 = ctypes.c_int64

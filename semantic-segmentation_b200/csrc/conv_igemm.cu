@@ -342,6 +342,15 @@ static bool desc_ok(const b200seg_conv_desc* d) {
   return true;
 }
 
+// The halo-tile kernel (conv3x3_halo.cu) runs dense 3x3 stride-1 convolutions into a bf16 output whose channels tile by
+// 16: the forward's cout (which = 0) or the data gradient's cin (which = 1). Everything else, dilated 3x3 layers and
+// forced channel chunks included, runs the per-tap conv_igemm_kernel. Every launch entry point and the plan query ask
+// this one predicate, so the reported plan is the launched one.
+static bool halo_eligible(const b200seg_conv_desc* d, int which) {
+  if (d->ksize != 3 || d->stride != 1 || conv_dil(d) != 1 || d->reserved != 0) return false;
+  return which == 0 ? !d->out_fp32 && d->cout % 16 == 0 : d->cin % 16 == 0;
+}
+
 static int g_smem_reserve = 0;
 int smem_reserve() { return g_smem_reserve; }
 
@@ -519,13 +528,18 @@ extern "C" size_t b200seg_conv2d_stats_elems(const b200seg_conv_desc* d) {
 // Host-only: the launch plan of a forward (which = 0) or stride-1 data-gradient (which = 1) convolution, for tests and
 // tuning scripts. out[12] = {kernel (1 halo / 0 per-tap), BN, n_tiles, grid, dynamic smem bytes, ring depth, CTAs per SM,
 // accumulator registers per consumer thread, resident weights (halo), weight slots (halo), channel chunk, total tiles}.
+// With B200SEG_PLAN_WINDOW added to which, out holds 13 entries and out[12] is the statistics window (1: each CTA keeps
+// only its own N tile's statistics columns, the grid a multiple of n_tiles); callers of the 12-entry form never get it.
 extern "C" int b200seg_conv2d_plan_info(const b200seg_conv_desc* d, int32_t which, int32_t* out) {
+  const bool want_window = (which & B200SEG_PLAN_WINDOW) != 0;
+  which &= ~B200SEG_PLAN_WINDOW;
   if (!desc_ok(d) || !out || which < 0 || which > 1) return B200SEG_E_BADARG;
   if (which == 1 && d->stride != 1) return B200SEG_E_BADARG;
-  const bool halo_fwd = d->ksize == 3 && d->stride == 1 && !d->out_fp32 && d->cout % 16 == 0 && d->reserved == 0;
-  const bool halo_bwd = d->ksize == 3 && d->cin % 16 == 0 && d->reserved == 0;
-  if (which == 0 && halo_fwd) return conv3x3_halo_plan_info(d->n, d->h, d->w, d->cin, d->cout, out);
-  if (which == 1 && halo_bwd) return conv3x3_halo_plan_info(d->n, d->h, d->w, (d->cout + 7) / 8 * 8, d->cin, out);
+  if (halo_eligible(d, which)) {
+    if (want_window) out[12] = 0;     // the halo kernel keeps every channel's statistics in each CTA
+    return which == 0 ? conv3x3_halo_plan_info(d->n, d->h, d->w, d->cin, d->cout, out)
+                      : conv3x3_halo_plan_info(d->n, d->h, d->w, (d->cout + 7) / 8 * 8, d->cin, out);
+  }
   LaunchGeom g = fwd_geom(d);
   if (which == 1) {          // same GEMM shape with the channel roles swapped (taps and lattice as the forward)
     g.in_c = (d->cout + 7) / 8 * 8; g.in_ld = g.in_c; g.out_c = d->cin; g.out_ld = d->cin;
@@ -535,13 +549,14 @@ extern "C" int b200seg_conv2d_plan_info(const b200seg_conv_desc* d, int32_t whic
   if (int rc = plan_geom(g, &pl)) return rc;
   out[0] = 0; out[1] = pl.BN; out[2] = pl.n_tiles; out[3] = pl.grid; out[4] = (int32_t)pl.smem_bytes; out[5] = pl.nstages;
   out[6] = pl.occ; out[7] = pl.acc_regs; out[8] = 0; out[9] = 0; out[10] = pl.KC; out[11] = pl.total_tiles;
+  if (want_window) out[12] = pl.stat_window;
   return 0;
 }
 
 extern "C" int b200seg_conv2d_fwd(const b200seg_conv_desc* d, const void* x, const void* w_ohwi, const float* bias,
                                   void* y, float* stats_partials, int32_t* stats_grid, void* stream) {
   if (!desc_ok(d)) return B200SEG_E_BADARG;
-  if (d->ksize == 3 && d->stride == 1 && !d->out_fp32 && d->cout % 16 == 0 && d->reserved == 0 && conv_dil(d) == 1) {
+  if (halo_eligible(d, 0)) {
     if (d->emit_stats && !stats_partials) return B200SEG_E_BADARG;
     // halo-tile kernel: the input is read once per tile instead of once per filter tap (conv3x3_halo.cu)
     return conv3x3_halo_launch(d->n, d->h, d->w, d->cin, d->x_ld, x, d->cout, w_ohwi, d->has_bias ? bias : nullptr, y,
@@ -559,7 +574,7 @@ extern "C" int b200seg_set_smem_reserve(int32_t bytes) {
 extern "C" int b200seg_conv2d_fwd_bn(const b200seg_conv_desc* d, const void* x, const void* w_ohwi, const float* bias,
                                      void* y, const b200seg_bn_fold* fold, void* stream) {
   if (!desc_ok(d) || !fold || !d->emit_stats || d->out_fp32) return B200SEG_E_BADARG;
-  if (d->ksize == 3 && d->stride == 1 && d->cout % 16 == 0 && d->reserved == 0 && conv_dil(d) == 1)
+  if (halo_eligible(d, 0))
     return conv3x3_halo_launch(d->n, d->h, d->w, d->cin, d->x_ld, x, d->cout, w_ohwi, d->has_bias ? bias : nullptr, y,
                                d->y_ld, nullptr, nullptr, nullptr, 0, 1, (cudaStream_t)stream, fold);
   return launch_geom(fwd_geom(d), x, w_ohwi, bias, y, nullptr, nullptr, nullptr, 0, (cudaStream_t)stream, fold);
@@ -573,7 +588,7 @@ extern "C" int b200seg_conv2d_fwd_add(const b200seg_conv_desc* d, const void* x,
                                       int32_t* stats_grid, void* stream) {
   if (!desc_ok(d) || !addend || d->out_fp32) return B200SEG_E_BADARG;
   if (d->emit_stats && !stats_partials) return B200SEG_E_BADARG;
-  if (d->ksize == 3 && d->stride == 1 && d->cout % 16 == 0 && d->reserved == 0 && conv_dil(d) == 1)
+  if (halo_eligible(d, 0))
     return conv3x3_halo_launch(d->n, d->h, d->w, d->cin, d->x_ld, x, d->cout, w_ohwi, d->has_bias ? bias : nullptr, y,
                                d->y_ld, stats_partials, stats_grid, addend, addend_ld, d->emit_stats, (cudaStream_t)stream);
   return launch_geom(fwd_geom(d), x, w_ohwi, bias, y, stats_partials, stats_grid, addend, addend_ld, (cudaStream_t)stream);
@@ -590,7 +605,7 @@ extern "C" int b200seg_conv2d_fwd_affine(const b200seg_conv_desc* d, const void*
   fd.scale = const_cast<float*>(scale);
   fd.shift = const_cast<float*>(shift);
   fd.relu = relu ? 1 : 0;
-  if (d->ksize == 3 && d->stride == 1 && d->cout % 16 == 0 && d->reserved == 0 && conv_dil(d) == 1)
+  if (halo_eligible(d, 0))
     return conv3x3_halo_launch(d->n, d->h, d->w, d->cin, d->x_ld, x, d->cout, w_ohwi, nullptr, y, d->y_ld, nullptr,
                                nullptr, addend, addend_ld, 0, (cudaStream_t)stream, nullptr, &fd);
   return launch_geom(fwd_geom(d), x, w_ohwi, nullptr, y, nullptr, nullptr, addend, addend_ld, (cudaStream_t)stream,
@@ -613,7 +628,7 @@ extern "C" int b200seg_conv2d_dgrad(const b200seg_conv_desc* d, const void* dy, 
   g.out_h = d->h; g.out_w = d->w; g.out_c = d->cin; g.out_ld = dx_ld;
   g.in_stride = 1; g.wtaps = taps;
   g.out_fp32 = 0; g.has_bias = 0; g.emit_stats = 0; g.force_kc = d->reserved;
-  if (d->stride == 1 && K == 3 && d->cin % 16 == 0 && d->reserved == 0 && dil == 1)
+  if (halo_eligible(d, 1))
     return conv3x3_halo_launch(d->n, d->h, d->w, g.in_c, dy_ld, dy, d->cin, w_dgrad, nullptr, dx, dx_ld, nullptr, nullptr,
                                addend, addend_ld, 0, (cudaStream_t)stream);
   if (d->stride == 1) {

@@ -21,34 +21,40 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 P, B = 1386.7e12, 6650e9
 
 
-def load_trace():
+def load_trace(args=(), descriptors=False):
+    """(kernel name, kind, detail, flops, bytes) per expected tensor-core kernel launch of the program
+    tools/trace_step.py traces with the command-line arguments args; descriptors=True appends the launch's descriptor
+    ((n, h, w, cin, cout, k, stride, dilation), emit_stats, out_fp32, has_bias)."""
     spec = importlib.util.spec_from_file_location("trace_step", os.path.join(ROOT, "tools", "trace_step.py"))
     ts = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(ts)
-    argv, sys.argv = sys.argv, ["trace_step.py"]
+    argv, sys.argv = sys.argv, ["trace_step.py"] + list(args)
     stdout, sys.stdout = sys.stdout, open(os.devnull, "w")
     try:
         ts.main()
     finally:
         sys.stdout, sys.argv = stdout, argv
-    exp = []        # (kernel name, kind, detail, flops, bytes) per expected tensor-core kernel launch
-    for name, nbytes, flops, detail in ts.EVENTS:
-        m = re.match(r"(\d+)x(\d+) c(\d+)->(\d+) k(\d) s(\d)", detail or "")
+    exp = []
+    for i, (name, nbytes, flops, detail) in enumerate(ts.EVENTS):
+        m = re.match(r"(\d+)x(\d+) c(\d+)->(\d+) k(\d) s(\d)(?: d(\d+))?$", detail or "")
         if not m:
             continue
-        h, w, cin, cout, k, s = map(int, m.groups())
+        h, w, cin, cout, k, s = map(int, m.groups()[:6])
+        dense = m.group(7) is None          # dilated 3x3 layers run the per-tap kernel (conv_igemm.cu halo_eligible)
+        desc = ts.CONV_DESCS[i]
+        tail = (desc,) if descriptors else ()
         if name.startswith("conv2d_fwd"):
-            halo = k == 3 and s == 1 and cout % 16 == 0 and cout != 19 and cout != 1
-            exp.append(("conv3x3_halo_kernel" if halo else "conv_igemm_kernel", "fwd", detail, flops, nbytes))
+            halo = k == 3 and s == 1 and dense and cout % 16 == 0 and not desc[2]
+            exp.append(("conv3x3_halo_kernel" if halo else "conv_igemm_kernel", "fwd", detail, flops, nbytes) + tail)
         elif name == "conv2d_dgrad":
-            if k == 3 and s == 1 and cin % 16 == 0:
-                exp.append(("conv3x3_halo_kernel", "dgrad", detail, flops, nbytes))
+            if k == 3 and s == 1 and dense and cin % 16 == 0:
+                exp.append(("conv3x3_halo_kernel", "dgrad", detail, flops, nbytes) + tail)
             else:
                 reps = 4 if (k == 3 and s == 2) else 1
                 for _ in range(reps):
-                    exp.append(("conv_igemm_kernel", "dgrad", detail, flops / reps, nbytes / reps))
+                    exp.append(("conv_igemm_kernel", "dgrad", detail, flops / reps, nbytes / reps) + tail)
         elif name == "conv2d_wgrad":
-            exp.append(("wgrad_igemm_kernel", "wgrad", detail, flops, nbytes))
+            exp.append(("wgrad_igemm_kernel", "wgrad", detail, flops, nbytes) + tail)
     return exp
 
 

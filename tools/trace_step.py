@@ -5,6 +5,7 @@ sum_launches max(FLOPs / P, bytes / B). Host-only planner queries (stats_elems, 
 library, so buffer sizes are the real ones.
 
     python -O tools/trace_step.py [--arch ocrnet.HRNet_Mscale] [--height 1024 --width 2048] [--tflops 1386.7 --gbs 6650]
+    python -O tools/trace_step.py --eval [--arch ...]      # the evaluation forwards at 0.5x, 1.0x and 2.0x instead
 
 -O is required: the wrappers assert `is_cuda`, and the point of this tool is to run them without a device.
 Bytes of a launch = sizes of the tensors handed to it (views count with their own extent), i.e. what the kernel must at
@@ -26,6 +27,8 @@ from b200seg import _lib, engine as EN, model as M, raw  # noqa: E402
 QUERY = re.compile(r"(_elems|_ws_bytes|_grid|_launches|_chunk|_splits|_abi_version|_build_info|_plan_info)$")
 SIZES = {}          # fake address -> bytes
 EVENTS = []         # (entry point, bytes, flops, detail)
+CONV_DESCS = {}     # index into EVENTS -> ((n, h, w, cin, cout, k, stride, dilation), emit_stats, out_fp32, has_bias):
+                    # the descriptor of a convolution as the step hands it over (a data gradient's cout is padded)
 _next = [0x7F0000000000]     # far above any scalar argument (pixel counts, pitches ...) the entry points take
 
 
@@ -61,6 +64,10 @@ class Recorder:
                         wo = (obj.w + 2 * obj.pad - dil * (k - 1) - 1) // s + 1
                         flops = 2.0 * obj.n * ho * wo * obj.cin * obj.cout * k * k
                         detail = "%dx%d c%d->%d k%d s%d" % (obj.h, obj.w, obj.cin, obj.cout, k, s)
+                        if dil > 1:
+                            detail += " d%d" % dil
+                        CONV_DESCS[len(EVENTS)] = ((obj.n, obj.h, obj.w, obj.cin, obj.cout, k, s, dil),
+                                                   obj.emit_stats, obj.out_fp32, obj.has_bias)
                     elif isinstance(obj, ctypes.c_int32):
                         obj.value = 148                       # stats_grid of the convolutions
             EVENTS.append((name[len("b200seg_"):], nbytes, flops, detail))
@@ -91,6 +98,9 @@ def main():
     ap.add_argument("--attn-head", default="default", choices=["default", "no3x3", "dropout", "oldarch", "no3x3_dropout"],
                     help="attention-head ablation of the multi-scale archs (--mscale_no3x3 / --mscale_dropout / "
                          "--mscale_old_arch of the reference's train.py)")
+    ap.add_argument("--eval", action="store_true",
+                    help="trace the evaluation forward instead of the training step: BatchNorm from the running "
+                         "statistics, one scale pass each at 0.5x, 1.0x and 2.0x of --height x --width")
     args = ap.parse_args()
     if __debug__:
         sys.exit("run with python -O (the wrappers assert is_cuda)")
@@ -120,6 +130,19 @@ def main():
         else:
             grads[n] = torch.empty(p.shape, dtype=torch.float32, device=dev)
     images = torch.empty((1, 3, args.height, args.width), dtype=torch.float32, device=dev)
+    if args.eval:
+        E = EN.Engine(tensors, {}, packed, False, None)
+        E.eval_bn = {n[: -len(".running_mean")]: (torch.empty(v.shape, dtype=torch.float32, device=dev),
+                                                  torch.empty(v.shape, dtype=torch.float32, device=dev))
+                     for n, v in tensors.items() if n.endswith(".running_mean")}
+        for s in (0.5, 1.0, 2.0):
+            hw = (int(args.height * s), int(args.width * s))
+            if A.has_wrn38_trunk(args.arch) and not A.is_two_scale(args.arch):
+                M.deepv3_pass(E, images, net.hcfg, hw, None)
+            else:
+                M.scale_pass(E, images, hw, args.arch, net.hcfg, net.ocfg)
+        report(args, "evaluation forward at 0.5x, 1.0x and 2.0x: %d launches" % len(EVENTS))
+        return
     gts = torch.empty((1, args.height, args.width), dtype=torch.long, device=dev)
     if A.has_wrn38_trunk(args.arch):
         n_sets = 2 if A.is_two_scale(args.arch) else 1        # one Dropout2d mask set per scale pass
@@ -137,7 +160,10 @@ def main():
     M.train_loss(E, images, gts, args.arch, net.hcfg, net.ocfg)
     n_fwd = len(EVENTS)
     M.run_backward(E)
+    report(args, "one crop: %d launches (%d forward + loss, %d backward)" % (len(EVENTS), n_fwd, len(EVENTS) - n_fwd))
 
+
+def report(args, what):
     P, B = args.tflops * 1e12, args.gbs * 1e9
     agg = collections.OrderedDict()
     tot = [0, 0.0, 0.0, 0.0]
@@ -146,8 +172,7 @@ def main():
         a = agg.setdefault(name, [0, 0.0, 0.0, 0.0])
         for acc in (a, tot):
             acc[0] += 1; acc[1] += flops; acc[2] += nbytes; acc[3] += t
-    print("%s  %dx%d  one crop: %d launches (%d forward + loss, %d backward)" %
-          (args.arch, args.height, args.width, len(EVENTS), n_fwd, len(EVENTS) - n_fwd))
+    print("%s  %dx%d  %s" % (args.arch, args.height, args.width, what))
     print("%-24s %8s %12s %12s %12s" % ("entry point", "launches", "TFLOP", "GB", "roofline ms"))
     for name, (c, f, b, t) in sorted(agg.items(), key=lambda kv: -kv[1][3]):
         print("%-24s %8d %12.3f %12.2f %12.3f" % (name, c, f / 1e12, b / 1e9, t * 1e3))
