@@ -6,6 +6,8 @@ library, so buffer sizes are the real ones.
 
     python -O tools/trace_step.py [--arch ocrnet.HRNet_Mscale] [--height 1024 --width 2048] [--tflops 1386.7 --gbs 6650]
     python -O tools/trace_step.py --eval [--arch ...]      # the evaluation forwards at 0.5x, 1.0x and 2.0x instead
+    python -O tools/trace_step.py --eval --assembly        # ... as b200seg.evaltail.eval_minibatch runs them, with the
+                                                           # output assembly, flips and the scoring tail
 
 -O is required: the wrappers assert `is_cuda`, and the point of this tool is to run them without a device.
 Bytes of a launch = sizes of the tensors handed to it (views count with their own extent), i.e. what the kernel must at
@@ -29,6 +31,10 @@ SIZES = {}          # fake address -> bytes
 EVENTS = []         # (entry point, bytes, flops, detail)
 CONV_DESCS = {}     # index into EVENTS -> ((n, h, w, cin, cout, k, stride, dilation), emit_stats, out_fp32, has_bias):
                     # the descriptor of a convolution as the step hands it over (a data gradient's cout is padded)
+LAUNCH_ARGS = {}    # index into EVENTS -> the arguments of every other launch (tools/ew_classes.py keys them): scalars as
+                    # they are, pointers as PTR (present) or None (absent), a fuse descriptor as ("fuse", n, h, w, c,
+                    # relu, ((h, w, ld, affine) per term)), a BatchNorm fold as ("fold", c, count, gamma, running, batch)
+PTR = "ptr"
 _next = [0x7F0000000000]     # far above any scalar argument (pixel counts, pitches ...) the entry points take
 
 
@@ -52,11 +58,20 @@ class Recorder:
 
         def fake(*args):
             nbytes, flops, detail = 0, 0.0, ""
+            rec = []
             for a in args:
                 if isinstance(a, int) and a in SIZES:
                     nbytes += SIZES[a]
+                    rec.append(PTR)
                 elif hasattr(a, "_obj"):                      # ctypes.byref(...)
                     obj = a._obj
+                    rec.append(PTR)                           # any other descriptor (a SyncBN exchange ...)
+                    if isinstance(obj, _lib.FuseDesc):
+                        rec[-1] = ("fuse", obj.n, obj.h, obj.w, obj.c, obj.relu,
+                                   tuple((t.h, t.w, t.ld, bool(t.scale)) for t in obj.term[:obj.nterms]))
+                    elif isinstance(obj, _lib.BnFold):
+                        rec[-1] = ("fold", obj.c, obj.count, bool(obj.gamma), bool(obj.running_mean),
+                                   bool(obj.batch_stats_out))
                     if isinstance(obj, _lib.ConvDesc):
                         k, s = obj.ksize, obj.stride
                         dil = max(1, getattr(obj, "dilation", 1))
@@ -70,6 +85,10 @@ class Recorder:
                                                    obj.emit_stats, obj.out_fp32, obj.has_bias)
                     elif isinstance(obj, ctypes.c_int32):
                         obj.value = 148                       # stats_grid of the convolutions
+                else:
+                    rec.append(a)
+            if not detail:
+                LAUNCH_ARGS[len(EVENTS)] = tuple(rec)
             EVENTS.append((name[len("b200seg_"):], nbytes, flops, detail))
             return 0
         return fake
@@ -101,6 +120,10 @@ def main():
     ap.add_argument("--eval", action="store_true",
                     help="trace the evaluation forward instead of the training step: BatchNorm from the running "
                          "statistics, one scale pass each at 0.5x, 1.0x and 2.0x of --height x --width")
+    ap.add_argument("--assembly", action="store_true",
+                    help="with --eval: run the evaluation as b200seg.evaltail.eval_minibatch does, with flips and the "
+                         "output assembly of b200seg.evalpath (multi-scale archs: N_SCALES 0.5, 1.0, 2.0 inside the "
+                         "network; the others: scales 0.5, 1.0, 2.0 around it)")
     args = ap.parse_args()
     if __debug__:
         sys.exit("run with python -O (the wrappers assert is_cuda)")
@@ -135,6 +158,13 @@ def main():
         E.eval_bn = {n[: -len(".running_mean")]: (torch.empty(v.shape, dtype=torch.float32, device=dev),
                                                   torch.empty(v.shape, dtype=torch.float32, device=dev))
                      for n, v in tensors.items() if n.endswith(".running_mean")}
+        if args.assembly:
+            from b200seg import evaltail
+            evaltail.eval_minibatch(_EvalNet(net, tensors, packed, E.eval_bn), images,
+                                    torch.empty((1, args.height, args.width), dtype=torch.long, device=dev),
+                                    scales=(0.5, 1.0, 2.0), do_flip=True)
+            report(args, "evaluation with output assembly: %d launches" % len(EVENTS))
+            return
         for s in (0.5, 1.0, 2.0):
             hw = (int(args.height * s), int(args.width * s))
             if A.has_wrn38_trunk(args.arch) and not A.is_two_scale(args.arch):
@@ -161,6 +191,26 @@ def main():
     n_fwd = len(EVENTS)
     M.run_backward(E)
     report(args, "one crop: %d launches (%d forward + loss, %d backward)" % (len(EVENTS), n_fwd, len(EVENTS) - n_fwd))
+
+
+class _EvalNet:
+    """What b200seg.evalpath.eval_forward and b200seg.evaltail.eval_minibatch read of a B200SegModule in eval mode, over
+    the traced meta tensors."""
+    training = False
+    lo_scale = 0.5
+
+    def __init__(self, net, tensors, packed, eval_bn):
+        from b200seg import arch as A
+        self.arch, self.hcfg, self.ocfg = net.arch, net.hcfg, net.ocfg
+        self.n_scales = (0.5, 1.0, 2.0) if A.is_two_scale(net.arch) else None
+        self._tensors = lambda: tensors
+        self._packed = packed
+        self._eval_bn_params = lambda: eval_bn
+        self._ensure_device_state = self._repack = lambda: None
+
+    def __call__(self, inputs):
+        from b200seg import evalpath
+        return evalpath.eval_forward(self, inputs["images"])
 
 
 def report(args, what):
