@@ -237,7 +237,9 @@ int b200seg_bn_running_update(float* running, const float* batch_pass0, const fl
 /* Multi-tensor SGD step (the update rule of the optimizer loss/optimizer.py:43-60 builds: momentum, weight decay,
  * optional nesterov) for every parameter of a group in ONE launch. items: DEVICE array; block b updates
  * b200seg_sgd_chunk() consecutive elements of items[blk_item[b]] from blk_start[b]. first_step: momentum buffers are
- * initialised with the (decayed) gradient. SURVEY.md §8(f) row f3. */
+ * initialised with the (decayed) gradient; it holds for every block of the launch, so a group whose parameters got their
+ * first gradient at different steps needs one launch for the fresh blocks and one for the others. SURVEY.md §8(f) row
+ * f3. */
 typedef struct b200seg_sgd_item {
   void* param;             /* fp32 [numel] */
   const void* grad;        /* fp32 [numel] */

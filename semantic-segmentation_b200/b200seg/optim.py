@@ -27,7 +27,9 @@ class FusedSGD(torch.optim.Optimizer):
         old = {id(p): self.state[p]["momentum_buffer"].clone() for p in ps if "momentum_buffer" in self.state.get(p, {})}
         flat = torch.zeros(total, dtype=torch.float32, device=dev)
         chunk = lib().b200seg_sgd_chunk()
-        items, blk_item, blk_start = [], [], []
+        # blocks of the parameters without a momentum buffer come first: their first update starts the buffer at the
+        # gradient (torch.optim.SGD), whatever buffers the group's other parameters already hold
+        items, blocks = [], ([], [])
         off = 0
         for i, p in enumerate(ps):
             assert p.is_cuda and p.dtype == torch.float32 and p.is_contiguous() and p.grad.is_contiguous()
@@ -36,15 +38,15 @@ class FusedSGD(torch.optim.Optimizer):
                 buf.copy_(old[id(p)])
             self.state[p]["momentum_buffer"] = buf
             items.append((p.data_ptr(), p.grad.data_ptr(), buf.data_ptr(), p.numel()))
-            for st in range(0, p.numel(), chunk):
-                blk_item.append(i)
-                blk_start.append(st)
+            blocks[id(p) in old].extend((i, st) for st in range(0, p.numel(), chunk))
             off += (p.numel() + 63) // 64 * 64
+        blk_item = [i for i, _st in blocks[0] + blocks[1]]
+        blk_start = [st for _i, st in blocks[0] + blocks[1]]
         it_np = np.array(items, dtype=np.dtype([("p", "<u8"), ("g", "<u8"), ("m", "<u8"), ("n", "<i8")]))
         tab = dict(key=key, items=torch.from_numpy(it_np.view(np.uint8).copy()).to(dev),
                    blk_item=torch.tensor(blk_item, dtype=torch.int32, device=dev),
                    blk_start=torch.tensor(blk_start, dtype=torch.int32, device=dev), n_blocks=len(blk_item),
-                   fresh=not old, flat=flat)
+                   n_fresh=len(blocks[0]), flat=flat)
         self._tables[gi] = tab
         return tab
 
@@ -55,9 +57,12 @@ class FusedSGD(torch.optim.Optimizer):
             if not any(p.grad is not None for p in group["params"]):
                 continue
             tab = self._table(gi, group)
-            check(lib().b200seg_sgd_step(ptr(tab["items"]), ptr(tab["blk_item"]), ptr(tab["blk_start"]), tab["n_blocks"],
-                                         float(group["lr"]), float(group["momentum"]), float(group["dampening"]),
-                                         float(group["weight_decay"]), int(group["nesterov"]), int(tab["fresh"]),
-                                         stream_ptr()), "sgd_step")
-            tab["fresh"] = False
+            nf = tab["n_fresh"]
+            for first, lo, hi in ((1, 0, nf), (0, nf, tab["n_blocks"])):
+                if hi > lo:
+                    check(lib().b200seg_sgd_step(ptr(tab["items"]), ptr(tab["blk_item"][lo:]), ptr(tab["blk_start"][lo:]),
+                                                 hi - lo, float(group["lr"]), float(group["momentum"]),
+                                                 float(group["dampening"]), float(group["weight_decay"]),
+                                                 int(group["nesterov"]), first, stream_ptr()), "sgd_step")
+            tab["n_fresh"] = 0
         return loss

@@ -23,30 +23,30 @@ def _programs():
     return [p + ["--assembly"] if "--eval" in p else p for p in conv_plans._programs()]
 
 
-_TRACE = """import importlib.util, json, os, sys
+_TRACE = """import importlib, importlib.util, json, os, sys
 sys.path.insert(0, %r)
-import ew_classes
+classes = importlib.import_module(sys.argv[1])
 spec = importlib.util.spec_from_file_location("trace_step", os.path.join(%r, "trace_step.py"))
 ts = importlib.util.module_from_spec(spec)
 spec.loader.exec_module(ts)
-sys.argv = ["trace_step.py"] + sys.argv[1:]
+sys.argv = ["trace_step.py"] + sys.argv[2:]
 stdout, sys.stdout = sys.stdout, open(os.devnull, "w")
 ts.main()
 sys.stdout = stdout
 keys = {}
 for i, args in sorted(ts.LAUNCH_ARGS.items()):
-    key = ew_classes.launch_key(ts.EVENTS[i][0], args)
+    key = classes.launch_key(ts.EVENTS[i][0], args)
     if key is not None:
         keys.setdefault(repr(key), repr(args))
 print(json.dumps(keys))
 """ % ((os.path.join(ROOT, "tools"),) * 2)
 
 
-@functools.lru_cache(maxsize=None)
-def _step_keys():
-    """{repr(key): (program, repr(arguments of its first launch))} over every program of _programs(), one process per
-    program (trace_step runs with -O), as many at once as there are CPUs."""
-    progs, running, keys = _programs(), [], {}
+def trace_keys(progs, key_module):
+    """{repr(key): (program, repr(arguments of its first launch))} over the programs (argument lists of
+    tools/trace_step.py), keyed by launch_key of tools/<key_module>.py; one process per program (trace_step runs with
+    -O), as many at once as there are CPUs."""
+    running, keys = [], {}
 
     def reap(proc, prog):
         out, err = proc.communicate(timeout=900)
@@ -56,11 +56,16 @@ def _step_keys():
     for prog in progs:
         if len(running) >= (os.cpu_count() or 4):
             reap(*running.pop(0))
-        running.append((subprocess.Popen([sys.executable, "-O", "-c", _TRACE] + prog, stdout=subprocess.PIPE,
-                                         stderr=subprocess.PIPE, text=True), prog))
+        running.append((subprocess.Popen([sys.executable, "-O", "-c", _TRACE, key_module] + prog,
+                                         stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True), prog))
     while running:
         reap(*running.pop(0))
     return keys
+
+
+@functools.lru_cache(maxsize=None)
+def _step_keys():
+    return trace_keys(_programs(), "ew_classes")
 
 
 def _row_keys():

@@ -14,8 +14,9 @@ PTR = "ptr"
 SMS = 132                 # B200SEG_MAX_CTAS
 MAX_GRID = 264            # B200SEG_MAX_GRID
 
-# Entry points with their own oracle tests or outside this table: convolutions (tests/test_gpu_conv_classes.py), losses
-# (mscale_loss / RMI oracle tests), the optimizer and gradient bookkeeping, weight packing and the input pipeline.
+# Entry points outside this table: convolutions (tools/conv_classes.py, tests/test_gpu_conv_classes.py), the losses
+# (tools/loss_classes.py, tests/test_gpu_loss_classes.py), the optimizer, gradient bookkeeping and weight packing
+# (tests/test_gpu_bookkeeping.py) and the input pipeline (tests/test_gpu_augment.py).
 OUT_OF_SCOPE = frozenset([
     "conv2d_fwd", "conv2d_fwd_add", "conv2d_fwd_bn", "conv2d_fwd_affine", "conv2d_dgrad", "conv2d_wgrad",
     "pack_weight", "pack_weights", "grad_fold", "publish_grads", "sgd_step", "accum_f32", "bn_running_update",

@@ -8,6 +8,7 @@ library, so buffer sizes are the real ones.
     python -O tools/trace_step.py --eval [--arch ...]      # the evaluation forwards at 0.5x, 1.0x and 2.0x instead
     python -O tools/trace_step.py --eval --assembly        # ... as b200seg.evaltail.eval_minibatch runs them, with the
                                                            # output assembly, flips and the scoring tail
+    python -O tools/trace_step.py --criterion rmi --ocr-aux-rmi [--sup-wt 0.05]   # the training step with another loss
 
 -O is required: the wrappers assert `is_cuda`, and the point of this tool is to run them without a device.
 Bytes of a launch = sizes of the tensors handed to it (views count with their own extent), i.e. what the kernel must at
@@ -33,7 +34,8 @@ CONV_DESCS = {}     # index into EVENTS -> ((n, h, w, cin, cout, k, stride, dila
                     # the descriptor of a convolution as the step hands it over (a data gradient's cout is padded)
 LAUNCH_ARGS = {}    # index into EVENTS -> the arguments of every other launch (tools/ew_classes.py keys them): scalars as
                     # they are, pointers as PTR (present) or None (absent), a fuse descriptor as ("fuse", n, h, w, c,
-                    # relu, ((h, w, ld, affine) per term)), a BatchNorm fold as ("fold", c, count, gamma, running, batch)
+                    # relu, ((h, w, ld, affine) per term)), a BatchNorm fold as ("fold", c, count, gamma, running, batch),
+                    # a loss descriptor as ("ms", n, h, w, hq, wq, hm, wm, hl, wl, nheads, sup_wt, ignore_index, loss_kind)
 PTR = "ptr"
 _next = [0x7F0000000000]     # far above any scalar argument (pixel counts, pitches ...) the entry points take
 
@@ -72,6 +74,9 @@ class Recorder:
                     elif isinstance(obj, _lib.BnFold):
                         rec[-1] = ("fold", obj.c, obj.count, bool(obj.gamma), bool(obj.running_mean),
                                    bool(obj.batch_stats_out))
+                    elif isinstance(obj, _lib.MscaleDesc):
+                        rec[-1] = ("ms", obj.n, obj.h, obj.w, obj.hq, obj.wq, obj.hm, obj.wm, obj.hl, obj.wl,
+                                   obj.nheads, obj.sup_wt, obj.ignore_index, obj.loss_kind)
                     if isinstance(obj, _lib.ConvDesc):
                         k, s = obj.ksize, obj.stride
                         dil = max(1, getattr(obj, "dilation", 1))
@@ -124,6 +129,12 @@ def main():
                     help="with --eval: run the evaluation as b200seg.evaltail.eval_minibatch does, with flips and the "
                          "output assembly of b200seg.evalpath (multi-scale archs: N_SCALES 0.5, 1.0, 2.0 inside the "
                          "network; the others: scales 0.5, 1.0, 2.0 around it)")
+    ap.add_argument("--criterion", default="ce",
+                    help="loss of the training step, as B200SegModule takes it: ce, rmi or img_wt[:upper_bound[:half]]")
+    ap.add_argument("--sup-wt", type=float, default=0.0,
+                    help="supervised_mscale_wt of the two-scale archs (cfg.LOSS.SUPERVISED_MSCALE_WT)")
+    ap.add_argument("--ocr-aux-rmi", action="store_true",
+                    help="with --criterion rmi: RMI on the OCR auxiliary head too (cfg.LOSS.OCR_AUX_RMI)")
     args = ap.parse_args()
     if __debug__:
         sys.exit("run with python -O (the wrappers assert is_cuda)")
@@ -139,7 +150,8 @@ def main():
     flags = dict(no3x3=dict(mscale_inner_3x3=False), dropout=dict(mscale_dropout=True),
                  oldarch=dict(mscale_oldarch=True),
                  no3x3_dropout=dict(mscale_inner_3x3=False, mscale_dropout=True)).get(args.attn_head, {})
-    net = B200SegModule(args.arch, 19, ocfg=dict(A.OCR_DEFAULT, **flags))
+    net = B200SegModule(args.arch, 19, criterion=args.criterion, ocfg=dict(A.OCR_DEFAULT, **flags),
+                        supervised_mscale_wt=args.sup_wt, ocr_aux_rmi=args.ocr_aux_rmi)
     dev = torch.device("meta")
     tensors = {k: torch.empty(v.shape, dtype=v.dtype, device=dev) for k, v in net._tensors().items()}
     packed, grads = {}, {}
@@ -187,7 +199,8 @@ def main():
                    for n, v in tensors.items() if n.endswith(".running_mean")}
     E = EN.Engine(tensors, grads, packed, True, mask, bncells=bncells,
                   attn_seed=torch.empty((1,), dtype=torch.int64, device=dev))
-    M.train_loss(E, images, gts, args.arch, net.hcfg, net.ocfg)
+    M.train_loss(E, images, gts, args.arch, net.hcfg, net.ocfg, net.lo_scale, net.ocr_alpha, net.sup_wt,
+                 net.ignore_index, loss_kind=net.loss_kind, img_wt=net.img_wt, ocr_aux_rmi=net.ocr_aux_rmi)
     n_fwd = len(EVENTS)
     M.run_backward(E)
     report(args, "one crop: %d launches (%d forward + loss, %d backward)" % (len(EVENTS), n_fwd, len(EVENTS) - n_fwd))
