@@ -52,7 +52,20 @@ typedef struct b200seg_conv_desc {
   int32_t reserved;
   int32_t dilation;        /* 0 or 1: dense; d > 1: 3x3 taps d pixels apart, pad must equal d (WideResNet-38 mod5-7, ASPP:
                               network/wider_resnet.py:322-330, network/utils.py:176-192) */
+  const void* w_planes;    /* NULL, or the plane-ordered weight image of the launch (below): read instead of the weight
+                              operand by launches that run the halo-tile kernel, ignored by all others */
+  int32_t w_planes_rows;   /* rows of w_planes (b200seg_conv2d_planes_elems) */
 } b200seg_conv_desc;
+
+/* Plane-ordered weight image of a halo-tile launch: the same bf16 weights as the launch's operand ([Cout][9][Cin]: the
+ * forward's w_ohwi, or for the data gradient w_dgrad with Cout = the forward's cin and Cin = roundup8(the forward's cout)),
+ * stored as [tap][G = roundup16(Cin) / 8][rows][8 channels]: element (co, tap, ci) at ((tap G + ci / 8) rows + co) 8 +
+ * ci % 8. Each 8-channel plane of a tap is one contiguous run of rows x 16 bytes, so the kernel fills a (chunk, tap, Cout
+ * tile) weight tile with one bulk copy per plane. rows >= Cout covers every Cout tiling the kernel may pick; rows past Cout
+ * and channels past Cin must be zero (zero the image once; the pack kernels never write them). 16-byte aligned.
+ * Returns the image's element count 9 G 8 rows and *rows, or 0 when the launch (which = 0 forward, 1 stride-1 data
+ * gradient) does not run on the halo-tile kernel. Host only. */
+int64_t b200seg_conv2d_planes_elems(const b200seg_conv_desc* d, int32_t which, int32_t* rows);
 
 /* Host-only introspection of the launch plan (tests, tuning): which = 0 forward, 1 stride-1 data gradient; the kernel
  * reported is the one the launch entry points run for the same descriptor (dilation, out_fp32 and emit_stats count).
@@ -150,6 +163,16 @@ typedef struct b200seg_pack_item {
 int32_t b200seg_pack_chunk(void);
 int b200seg_pack_weights(const b200seg_pack_item* items, const int32_t* blk_item, const int32_t* blk_start,
                          int32_t n_blocks, int32_t which, void* stream);
+/* The same, also writing the plane-ordered weight images (b200seg_conv2d_planes_elems) of the 3x3 items: planes is a
+ * DEVICE array parallel to items; NULL image pointers are skipped (which & 1: fwd, which & 2: dgrad). */
+typedef struct b200seg_pack_planes {
+  void* fwd;               /* image of w_ohwi: Cin = i_dst, rows_fwd rows, or NULL */
+  void* dgrad;             /* image of w_dgrad: Cin = roundup8(o), rows_dgrad rows, or NULL */
+  int32_t rows_fwd, rows_dgrad;
+} b200seg_pack_planes;
+int b200seg_pack_weights_planes(const b200seg_pack_item* items, const b200seg_pack_planes* planes,
+                                const int32_t* blk_item, const int32_t* blk_start, int32_t n_blocks, int32_t which,
+                                void* stream);
 
 /* Data gradient: dx[n,h,w,cin] = conv_transpose(dy, W) (+ addend, e.g. a gradient that already arrived at x).
  * d describes the FORWARD convolution; dy: bf16 [n,ho,wo,*] whose channel extent is roundup8(cout) (pad channels

@@ -24,7 +24,8 @@ P32 = ctypes.POINTER(c_int32)
 class ConvDesc(ctypes.Structure):
     _fields_ = [(n, c_int32) for n in (
         "n", "h", "w", "cin", "cout", "ksize", "stride", "pad", "x_ld", "y_ld",
-        "out_fp32", "has_bias", "emit_stats", "reserved", "dilation")]
+        "out_fp32", "has_bias", "emit_stats", "reserved", "dilation")] + [
+        ("w_planes", c_void_p), ("w_planes_rows", c_int32)]     # plane-ordered weight image (include/b200seg.h)
 
 
 class FuseTerm(ctypes.Structure):
@@ -86,6 +87,8 @@ SIGNATURES = {
     "b200seg_pack_weight": (ctypes.c_int, [V, I32, I32, I32, V, V, I32, V]),
     "b200seg_pack_chunk": (I32, []),
     "b200seg_pack_weights": (ctypes.c_int, [V, V, V, I32, I32, V]),
+    "b200seg_pack_weights_planes": (ctypes.c_int, [V, V, V, V, I32, I32, V]),
+    "b200seg_conv2d_planes_elems": (ctypes.c_int64, [ctypes.POINTER(ConvDesc), c_int32, P32]),
     "b200seg_conv2d_dgrad": (ctypes.c_int, [ctypes.POINTER(ConvDesc), V, I32, V, V, I32, V, I32, V]),
     "b200seg_conv2d_wgrad_ws_bytes": (c_size_t, [ctypes.POINTER(ConvDesc)]),
     "b200seg_conv2d_wgrad_launches": (I32, [ctypes.POINTER(ConvDesc)]),

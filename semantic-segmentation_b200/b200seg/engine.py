@@ -52,7 +52,7 @@ class HeadRec:
 
 class Engine:
     def __init__(self, params, grads, packed, training, drop_mask=None, side_stream=None, bstat=None, stream=None,
-                 sync=None, pass_id=0, branch_streams=None, ws_holder=None, bncells=None, attn_seed=None):
+                 sync=None, pass_id=0, branch_streams=None, ws_holder=None, bncells=None, attn_seed=None, planes=None):
         """params: name -> tensor (weights, BN buffers); grads: name -> fp32 tensor accumulated into (training);
         packed: name -> (w_fwd, w_dgrad) bf16 operand caches; drop_mask: fp32 [N, mid] post-ReLU multiplier;
         bstat: BN layer name -> fp32 [2*C] slot receiving the batch [mean | unbiased var] (the running statistics are
@@ -65,10 +65,13 @@ class Engine:
         and the consuming apply pass folds them in its prologue (no finaliser launch on the chain; ignored with sync);
         branch_streams: up to three extra streams for the parallel branches of a HighResolutionModule (branch 0 stays
         on the engine's own stream); ws_holder: reusable weight-gradient slab workspace of the side stream;
-        attn_seed: int64 [1] device tensor, the step's key of the attention head's element-wise dropout (or None)."""
+        attn_seed: int64 [1] device tensor, the step's key of the attention head's element-wise dropout (or None);
+        planes: name -> (forward image, data-gradient image) plane-ordered copies of the packed operands that the
+        halo-tile launches stream their weights from (raw.planes_image; either may be None)."""
         self.p = params
         self.g = grads
         self.packed = packed
+        self.planes = planes or {}
         self.training = training
         self.drop_mask = drop_mask
         self.attn_seed = attn_seed
@@ -196,12 +199,14 @@ class Engine:
             if self.bstat is not None:
                 self.bn_seen.add(bname)
             rec.pending = self.bncells[bname][0]
-            rec.y = raw.conv2d_fwd_cells(x.t, w_f, b, stride, rec.pending, dilation=dilation)
+            rec.y = raw.conv2d_fwd_cells(x.t, w_f, b, stride, rec.pending, dilation=dilation,
+                                         planes=self._img(cname, 0))
             par = rec.par = raw._new((4, rec.cout), dtype=F32, device=x.t.device)
             rec.scale, rec.shift, rec.mean, rec.invstd = par[0], par[1], par[2], par[3]
             return rec
         if self.training:
-            y, stats = raw.conv2d_fwd(x.t, w_f, b, stride=stride, emit_stats=True, dilation=dilation)
+            y, stats = raw.conv2d_fwd(x.t, w_f, b, stride=stride, emit_stats=True, dilation=dilation,
+                                      planes=self._img(cname, 0))
             n, ho, wo, _ = y.shape
             if self.bstat is not None:
                 self.bn_seen.add(bname)
@@ -214,11 +219,14 @@ class Engine:
                                       self.p[bname + ".num_batches_tracked"], rec.cout, sync=self._sync(bname, 0))
             rec.scale, rec.shift, rec.mean, rec.invstd = par[0], par[1], par[2], par[3]
         else:
-            y = raw.conv2d_fwd(x.t, w_f, b, stride=stride, dilation=dilation)
+            y = raw.conv2d_fwd(x.t, w_f, b, stride=stride, dilation=dilation, planes=self._img(cname, 0))
             par = self.eval_bn[bname]
             rec.scale, rec.shift, rec.mean, rec.invstd = par[0], par[1], None, None
         rec.y = y
         return rec
+
+    def _img(self, cname, which):
+        return self.planes.get(cname, (None, None))[which]
 
     def _sync(self, bname, direction):
         return self.sync.args(self.pass_id, bname, direction) if self.sync is not None else None
@@ -234,11 +242,13 @@ class Engine:
         # a conv bias in front of a training-mode BN has an exactly zero gradient (BN removes the mean): left at 0
         if x.needs_grad:
             _, w_d = self.packed[rec.cname]
+            img = self._img(rec.cname, 1)
             if x.grad is None:
-                x.grad = raw.conv2d_dgrad(dy, w_d, tuple(x.t.shape), rec.ksize, rec.stride, dilation=rec.dil)
+                x.grad = raw.conv2d_dgrad(dy, w_d, tuple(x.t.shape), rec.ksize, rec.stride, dilation=rec.dil,
+                                          planes=img)
             else:
                 raw.conv2d_dgrad(dy, w_d, tuple(x.t.shape), rec.ksize, rec.stride, addend=x.grad, out=x.grad,
-                                 dilation=rec.dil)
+                                 dilation=rec.dil, planes=img)
 
     def bn_act(self, rec, relu=True, residual=None, out=None, post_scale=None, dropout=None):
         """dropout: (int64 [1] seed tensor, pass index) of an element-wise Dropout(0.5) after the ReLU, or None."""
@@ -281,7 +291,8 @@ class Engine:
             if bias:                 # (conv + b) * s + t = conv * s + (b * s + t)
                 shift = shift + self.p[cname + ".bias"].float() * scale
             z = raw.conv2d_fwd_affine(x.t, w_f, scale, shift, relu, stride=stride,
-                                      addend=residual.t if residual is not None else None, out=out, dilation=dilation)
+                                      addend=residual.t if residual is not None else None, out=out, dilation=dilation,
+                                      planes=self._img(cname, 0))
             return Act(z)
         rec = self.conv_stats(x, cname, bname, ksize, stride, bias, dilation, defer=True)
         return self.bn_act(rec, relu, residual, out, post_scale, dropout)
@@ -305,7 +316,7 @@ class Engine:
         cout = w_f.shape[0]
         stats = None
         res = raw.conv2d_fwd(x.t, w_f, None, stride=stride, emit_stats=want_stats and self.training, dilation=dilation,
-                             addend=addend.t if addend is not None else None, out=out)
+                             addend=addend.t if addend is not None else None, out=out, planes=self._img(cname, 0))
         if want_stats and self.training:
             y, stats = res
         else:
@@ -320,11 +331,12 @@ class Engine:
             self.wgrad(x.t, dy, self.g[cname + ".weight"], cout, ksize, stride, dilation)
             if x.needs_grad:
                 _, w_d = self.packed[cname]
+                img = self._img(cname, 1)
                 if x.grad is None:
-                    x.grad = raw.conv2d_dgrad(dy, w_d, tuple(x.t.shape), ksize, stride, dilation=dilation)
+                    x.grad = raw.conv2d_dgrad(dy, w_d, tuple(x.t.shape), ksize, stride, dilation=dilation, planes=img)
                 else:
                     raw.conv2d_dgrad(dy, w_d, tuple(x.t.shape), ksize, stride, addend=x.grad, out=x.grad,
-                                     dilation=dilation)
+                                     dilation=dilation, planes=img)
             if addend is not None:
                 self._add_grad(addend, dy)
             ya.grad = None

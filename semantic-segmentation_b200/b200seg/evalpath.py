@@ -42,7 +42,7 @@ def eval_forward(module, images):
     images = images.contiguous().float()
     n, _, H, W = images.shape
     tensors = {k: v.detach() for k, v in module._tensors().items()}
-    E = Engine(tensors, {}, module._packed, False, None)
+    E = Engine(tensors, {}, module._packed, False, None, planes=module._planes)
     # BatchNorm from running statistics: every layer's scale / shift up front; conv + BN (+ residual) + ReLU then run as
     # ONE launch each (raw.conv2d_fwd_affine).
     E.eval_bn = module._eval_bn_params()

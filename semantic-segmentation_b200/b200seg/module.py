@@ -156,6 +156,7 @@ class B200SegModule(nn.Module):
         self._build_parameters()
         self._flat_grad = None
         self._packed = None
+        self._planes = {}
         self._graphs = {}
         self._ddp_allreduce = False
         self._anchor = None
@@ -246,6 +247,9 @@ class B200SegModule(nn.Module):
                 self._grad_views[n] = self._flat_grad[off:off + p.numel()].view(p.shape)
                 off += (p.numel() + 63) // 64 * 64
             self._packed = {}
+            # plane-ordered copies of the 3x3 operands that the halo-tile kernel streams its weights from (contiguous
+            # bulk copies instead of 16-byte TMA rows), written by the same pack launch
+            self._planes = {}
             for n, p in params:
                 if p.dim() == 4:
                     o, i, k, _ = p.shape
@@ -254,6 +258,9 @@ class B200SegModule(nn.Module):
                     w_f = torch.zeros((o, k * k, i), dtype=torch.bfloat16, device=dev)
                     w_d = torch.zeros((i, k * k, (o + 7) // 8 * 8), dtype=torch.bfloat16, device=dev)
                     self._packed[n[: -len(".weight")]] = (w_f, w_d)
+                    imgs = tuple(raw.planes_image((o, i, k, k), which, dev) for which in (0, 1))
+                    if imgs != (None, None):
+                        self._planes[n[: -len(".weight")]] = imgs
             self._graphs = {}
             self._build_grad_accumulators(params, dev)
         self._ensure_flat_running(dev)
@@ -382,7 +389,8 @@ class B200SegModule(nn.Module):
         ptrs = tuple(p.data_ptr() for _, p in convs)
         tab = getattr(self, "_pack_table", None)
         if tab is None or tab["ptrs"] != ptrs:
-            entries = [(p.detach(), *self._packed[n[: -len(".weight")]]) for n, p in convs]
+            entries = [(p.detach(), *self._packed[n[: -len(".weight")]],
+                        *self._planes.get(n[: -len(".weight")], (None, None))) for n, p in convs]
             tab = self._pack_table = raw.pack_table(entries, convs[0][1].device)
             self._graphs = {}
         if side is None:
@@ -456,14 +464,14 @@ class B200SegModule(nn.Module):
             E_lo = Engine(tensors, grads_lo, self._packed, True, drop_mask, side_stream=self._side_stream_lo,
                           bstat=self._bstat_views[0], stream=self._lo_stream, sync=sync, pass_id=0,
                           branch_streams=self._bstreams["lo"], ws_holder=self._ws_holders["lo"],
-                          bncells=self._bncells[0] if use_cells else None, attn_seed=attn_seed)
+                          bncells=self._bncells[0] if use_cells else None, attn_seed=attn_seed, planes=self._planes)
         two_pass = A.is_two_scale(self.arch)
         if sync is not None and two_pass and not par:
             raise RuntimeError("SyncBN needs parallel_scales=True for the two-scale step (one engine per pass)")
         E = Engine(tensors, grads, self._packed, True, drop_mask, side_stream=self._side_stream,
                    bstat=self._bstat_views[1] if par else None, sync=sync, pass_id=1 if two_pass else 0,
                    branch_streams=self._bstreams["hi"], ws_holder=self._ws_holders["hi"],
-                   bncells=self._bncells[1] if use_cells else None, attn_seed=attn_seed)
+                   bncells=self._bncells[1] if use_cells else None, attn_seed=attn_seed, planes=self._planes)
         loss = M.train_loss(E, images, gts, self.arch, self.hcfg, self.ocfg, self.lo_scale, self.ocr_alpha, self.sup_wt,
                             self.ignore_index, E_lo=E_lo, loss_kind=self.loss_kind, img_wt=self.img_wt,
                             ocr_aux_rmi=self.ocr_aux_rmi)

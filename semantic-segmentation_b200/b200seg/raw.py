@@ -71,13 +71,38 @@ def pack_weight_into(w_oihw, w_f, w_d):
     check(lib().b200seg_pack_weight(ptr(w_oihw), o, i, k, ptr(w_f), ptr(w_d), o_pad, stream_ptr()), "pack_weight")
 
 
+def planes_image(w_shape, which, device):
+    """Zeroed plane-ordered weight image (include/b200seg.h) of a 3x3 layer with OIHW weight shape w_shape, as a stride-1
+    dense launch reads it (which = 0 forward, 1 data gradient): bf16 [9][G][rows][8], or None when that launch does not
+    run on the halo-tile kernel."""
+    o, i, k, _ = w_shape
+    if k != 3:
+        return None
+    d = conv_desc(1, 1, 1, i, (o + 7) // 8 * 8 if which else o, 3, 1, i, o)
+    rows = ctypes.c_int32(0)
+    n = lib().b200seg_conv2d_planes_elems(ctypes.byref(d), which, ctypes.byref(rows))
+    if n == 0:
+        return None
+    return torch.zeros((9, n // (72 * rows.value), rows.value, 8), dtype=BF16, device=device)
+
+
+def _set_planes(d, planes):
+    if planes is not None:
+        assert planes.dtype == BF16 and planes.is_contiguous() and planes.dim() == 4, planes.shape
+        d.w_planes, d.w_planes_rows = planes.data_ptr(), planes.shape[2]
+
+
 def pack_table(entries, device):
-    """entries: list of (w_oihw fp32 tensor, w_f, w_d) -> device tables for pack_weights (one launch for all of them).
-    The table stores raw pointers: rebuild it when a parameter's storage moves."""
+    """entries: list of (w_oihw fp32 tensor, w_f, w_d) or (w_oihw, w_f, w_d, planes_fwd, planes_dgrad) -> device tables
+    for pack_weights (one launch for all of them); the images (planes_image, either may be None) are written by the same
+    launch. The table stores raw pointers: rebuild it when a parameter's storage moves."""
     import numpy as np
     chunk = lib().b200seg_pack_chunk()
-    items, blk_item, blk_start = [], [], []
-    for idx, (w, w_f, w_d) in enumerate(entries):
+    items, blk_item, blk_start, planes = [], [], [], []
+    for idx, (w, w_f, w_d, *img) in enumerate(entries):
+        p_f, p_d = img if img else (None, None)
+        planes.append((p_f.data_ptr() if p_f is not None else 0, p_d.data_ptr() if p_d is not None else 0,
+                       p_f.shape[2] if p_f is not None else 0, p_d.shape[2] if p_d is not None else 0))
         o, i, k, _ = w.shape
         i_dst = w_f.shape[2]
         assert w.is_contiguous() and w.dtype == F32
@@ -88,14 +113,23 @@ def pack_table(entries, device):
             blk_start.append(st)
     it_np = np.array(items, dtype=np.dtype([("w", "<u8"), ("f", "<u8"), ("d", "<u8"), ("o", "<i4"), ("i", "<i4"),
                                             ("i_dst", "<i4"), ("k", "<i4"), ("o_pad", "<i4"), ("r", "<i4")]))
-    return dict(items=torch.from_numpy(it_np.view(np.uint8).copy()).to(device),
-                blk_item=torch.tensor(blk_item, dtype=torch.int32, device=device),
-                blk_start=torch.tensor(blk_start, dtype=torch.int32, device=device), n_blocks=len(blk_item),
-                ptrs=tuple(e[0].data_ptr() for e in entries))
+    tab = dict(items=torch.from_numpy(it_np.view(np.uint8).copy()).to(device),
+               blk_item=torch.tensor(blk_item, dtype=torch.int32, device=device),
+               blk_start=torch.tensor(blk_start, dtype=torch.int32, device=device), n_blocks=len(blk_item),
+               ptrs=tuple(e[0].data_ptr() for e in entries))
+    if any(pl[0] or pl[1] for pl in planes):
+        pl_np = np.array(planes, dtype=np.dtype([("f", "<u8"), ("d", "<u8"), ("rf", "<i4"), ("rd", "<i4")]))
+        tab["planes"] = torch.from_numpy(pl_np.view(np.uint8).copy()).to(device)
+    return tab
 
 
 def pack_weights(table, which=3):
-    """which: 1 forward operands, 2 data-gradient operands, 3 both."""
+    """which: 1 forward operands, 2 data-gradient operands, 3 both (each with its plane-ordered images)."""
+    if "planes" in table:
+        check(lib().b200seg_pack_weights_planes(ptr(table["items"]), ptr(table["planes"]), ptr(table["blk_item"]),
+                                                ptr(table["blk_start"]), table["n_blocks"], which, stream_ptr()),
+              "pack_weights")
+        return
     check(lib().b200seg_pack_weights(ptr(table["items"]), ptr(table["blk_item"]), ptr(table["blk_start"]),
                                      table["n_blocks"], which, stream_ptr()), "pack_weights")
 
@@ -118,8 +152,9 @@ def out_hw(h, w, ksize, stride, dilation=1):
 
 
 def conv2d_fwd(x, w_ohwi, bias=None, stride=1, out=None, out_fp32=False, emit_stats=False, force_kc=0,
-               direct=False, out_ld=None, dilation=1, addend=None):
-    """x: [N,H,W,Cin] bf16; w_ohwi: [Cout][k*k][Cin] bf16. Returns y (and with emit_stats the per-CTA partials
+               direct=False, out_ld=None, dilation=1, addend=None, planes=None):
+    """x: [N,H,W,Cin] bf16; w_ohwi: [Cout][k*k][Cin] bf16; planes: optional plane-ordered image of w_ohwi (planes_image),
+    read instead of it when the launch runs on the halo-tile kernel. Returns y (and with emit_stats the per-CTA partials
     [grid][2][cout_pad] fp32)."""
     assert x.is_cuda and x.dtype == BF16
     cout, taps, cin = w_ohwi.shape
@@ -133,6 +168,7 @@ def conv2d_fwd(x, w_ohwi, bias=None, stride=1, out=None, out_fp32=False, emit_st
         out = buf[..., :cout] if width != cout else buf
     d = conv_desc(n, h, w, cin, cout, ksize, stride, _ld(x), _ld(out), out_fp32, bias is not None, emit_stats,
                   force_kc, dilation)
+    _set_planes(d, planes)
     if direct:
         from ._lib import test_lib        # test-only library (tests/test_gpu_ops.py cross-check)
         check(test_lib().b200seg_conv2d_fwd_direct(ctypes.byref(d), ptr(x), ptr(w_ohwi), ptr(bias), ptr(out),
@@ -155,7 +191,7 @@ def conv2d_fwd(x, w_ohwi, bias=None, stride=1, out=None, out_fp32=False, emit_st
     return out
 
 
-def conv2d_fwd_affine(x, w_ohwi, scale, shift, relu, stride=1, addend=None, out=None, dilation=1):
+def conv2d_fwd_affine(x, w_ohwi, scale, shift, relu, stride=1, addend=None, out=None, dilation=1, planes=None):
     """Evaluation: y = relu?(conv(x) * scale + shift (+ addend)) in one launch (BatchNorm from running statistics)."""
     assert x.is_cuda and x.dtype == BF16
     cout, taps, cin = w_ohwi.shape
@@ -166,6 +202,7 @@ def conv2d_fwd_affine(x, w_ohwi, scale, shift, relu, stride=1, addend=None, out=
     if out is None:
         out = _new((n, ho, wo, cout), dtype=BF16, device=x.device)
     d = conv_desc(n, h, w, cin, cout, ksize, stride, _ld(x), _ld(out), dilation=dilation)
+    _set_planes(d, planes)
     check(lib().b200seg_conv2d_fwd_affine(ctypes.byref(d), ptr(x), ptr(w_ohwi), ptr(scale), ptr(shift), int(relu),
                                           ptr(addend), _ld(addend) if addend is not None else 0, ptr(out),
                                           stream_ptr()), "conv2d_fwd_affine")
@@ -183,7 +220,7 @@ def _cells_fold(cells, par, gamma, beta, eps, momentum, count, c, batch_out, run
     return f
 
 
-def conv2d_fwd_cells(x, w_ohwi, bias, stride, cells, out=None, dilation=1):
+def conv2d_fwd_cells(x, w_ohwi, bias, stride, cells, out=None, dilation=1, planes=None):
     """Convolution whose epilogue adds the batch statistics of the stored output to `cells` (fp64 [2*roundup16(cout)],
     zero at the start of the step) and nothing else: the consuming bn_apply_cells finalises them. Returns y."""
     assert x.is_cuda and x.dtype == BF16
@@ -196,6 +233,7 @@ def conv2d_fwd_cells(x, w_ohwi, bias, stride, cells, out=None, dilation=1):
         out = _new((n, ho, wo, cout), dtype=BF16, device=x.device)
     d = conv_desc(n, h, w, cin, cout, ksize, stride, _ld(x), _ld(out), False, bias is not None, True,
                   dilation=dilation)
+    _set_planes(d, planes)
     f = BnFold()
     f.accum, f.c = ptr(cells), cout
     check(lib().b200seg_conv2d_fwd_bn(ctypes.byref(d), ptr(x), ptr(w_ohwi), ptr(bias), ptr(out), ctypes.byref(f),
@@ -226,8 +264,9 @@ def bn_apply_cells(y, cells, par, gamma, beta, eps, momentum, res=None, post_sca
     return out
 
 
-def conv2d_dgrad(dy, w_dgrad, x_shape, ksize, stride, addend=None, out=None, force_kc=0, dilation=1):
-    """dy: [N,Ho,Wo,roundup8(Cout)] bf16; w_dgrad: [Cin][k*k][roundup8(Cout)]; x_shape = (N,H,W,Cin)."""
+def conv2d_dgrad(dy, w_dgrad, x_shape, ksize, stride, addend=None, out=None, force_kc=0, dilation=1, planes=None):
+    """dy: [N,Ho,Wo,roundup8(Cout)] bf16; w_dgrad: [Cin][k*k][roundup8(Cout)]; x_shape = (N,H,W,Cin); planes: optional
+    plane-ordered image of w_dgrad (planes_image with which = 1)."""
     n, h, w, cin = x_shape
     cout_pad = w_dgrad.shape[2]
     assert dy.shape[3] >= cout_pad or dy.shape[3] == cout_pad, (dy.shape, w_dgrad.shape)
@@ -239,6 +278,7 @@ def conv2d_dgrad(dy, w_dgrad, x_shape, ksize, stride, addend=None, out=None, for
         else:
             out = _new((n, h, w, cin), dtype=BF16, device=dy.device)
     d = conv_desc(n, h, w, cin, cout_pad, ksize, stride, _ld(out), _ld(out), force_kc=force_kc, dilation=dilation)
+    _set_planes(d, planes)
     check(lib().b200seg_conv2d_dgrad(ctypes.byref(d), ptr(dy), _ld(dy), ptr(w_dgrad), ptr(addend),
                                      _ld(addend) if addend is not None else 0, ptr(out), _ld(out), stream_ptr()),
           "conv2d_dgrad", (4 if ksize == 3 else 1) if stride == 2 else 1)

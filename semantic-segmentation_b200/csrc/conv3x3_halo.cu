@@ -9,6 +9,11 @@
 //     start = plane + (kh*10 + kw) * 16 B,   SBO = 10 * 16 B (next tile row),   LBO = plane pitch (next channel group)
 // The weights use the same no-swizzle layout ([channel group][BN][8 channels]). The last chunk of a Cin that is not a
 // multiple of 64 fetches only the planes its K steps read (both operands), not planes that lie wholly past Cin.
+// Weight source: a TMA box of BN 16-byte rows per plane from the [Cout][9][Cin] operand (rows 9 Cin x 2 B apart, so
+// every 16 bytes is its own L2 request), or, when the caller passes the plane-ordered image ([tap][Cin/8][rows][8],
+// include/b200seg.h), one contiguous 1-D bulk copy of BN x 16 bytes per plane: the same bytes at the same shared-memory
+// addresses, filled at L2 line rate. Each wgmma reads 128 pixels x BN x 16 channels against BN x 32 weight bytes, so a
+// streamed weight tile feeds only 128 FLOP per byte and the fill rate bounds the wide layers.
 //
 // Roles (288 threads): warps 0-7 = two consumer warpgroups (tile rows 0-7 / 8-15: MMA + epilogue), warp 8 = TMA producer.
 // Weights: resident in shared memory for the whole persistent CTA when they fit (C <= 96: the HBM-bound layers), else
@@ -45,6 +50,9 @@ struct HaloParams {
   int resident;                // weights stay in smem for the CTA lifetime
   int a_slots, b_slots;        // ring depths (b_slots unused when resident)
   int b_tile_bytes;            // BN * 128 rounded to 1024
+  const uint8_t* w_planes;     // plane-ordered weight image or null (TMA boxes of tmB)
+  size_t w_plane_bytes;        // image: rows x 16 B (one 8-channel plane of one tap)
+  size_t w_tap_bytes;          // image: roundup16(Cin) / 8 planes of one tap
 };
 
 constexpr int kHThreads = 288;
@@ -89,6 +97,16 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   // Channel-group planes fetched per chunk: the MMAs of a chunk with KS K steps read planes 0 .. 2 KS - 1 only, so the last
   // chunk of a Cin that is not a multiple of 64 skips the planes that would lie wholly past Cin (48: 2 of 8, 96: 4, 720: 6).
   const int planes_last = 2 * p.ksteps_last;
+  // weight planes 0 .. planes - 1 of (chunk cc, tap t, Cout tile n_tile) into dst, BN rows of 16 bytes per plane
+  auto load_w = [&](uint64_t* bar, uint8_t* dst, int cc, int t, int n_tile, int planes) {
+    if (p.w_planes) {
+      const uint8_t* src = p.w_planes + (size_t)t * p.w_tap_bytes + (size_t)(8 * cc) * p.w_plane_bytes +
+                           (size_t)n_tile * p.BN * 16;
+      for (int j = 0; j < planes; ++j) bulk_load(dst + j * p.BN * 16, src + (size_t)j * p.w_plane_bytes, p.BN * 16, bar);
+    } else {
+      for (int j = 0; j < planes; ++j) tma_load_3d(&tmB, bar, dst + j * p.BN * 16, cc * 64 + 8 * j, t, n_tile * p.BN);
+    }
+  };
   // Resident weights are static for the whole step (written by the pack kernels, which never trigger a programmatic
   // launch): fetch them while the previous kernel on the stream is still draining.
   if (warp == 8 && p.resident) {
@@ -96,9 +114,8 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       mbar_arrive_expect_tx(&b_full[0], 9 * ((p.cchunks - 1) * 8 + planes_last) * p.BN * 16);
       for (int cc = 0; cc < p.cchunks; ++cc)
         for (int t = 0; t < 9; ++t)
-          for (int j = 0; j < (cc == p.cchunks - 1 ? planes_last : 8); ++j)
-            tma_load_3d(&tmB, &b_full[0], b_base + (size_t)(cc * 9 + t) * p.b_tile_bytes + j * p.BN * 16, cc * 64 + 8 * j,
-                        t, 0);
+          load_w(&b_full[0], b_base + (size_t)(cc * 9 + t) * p.b_tile_bytes, cc, t, 0,
+                 cc == p.cchunks - 1 ? planes_last : 8);
     }
     __syncwarp();
   }
@@ -126,9 +143,7 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             for (int t = 0; t < 9; ++t) {
               mbar_wait(&b_empty[b_slot], b_phase ^ 1);
               mbar_arrive_expect_tx(&b_full[b_slot], planes * p.BN * 16);
-              for (int j = 0; j < planes; ++j)
-                tma_load_3d(&tmB, &b_full[b_slot], b_base + (size_t)b_slot * p.b_tile_bytes + j * p.BN * 16,
-                            cc * 64 + 8 * j, t, n_tile * p.BN);
+              load_w(&b_full[b_slot], b_base + (size_t)b_slot * p.b_tile_bytes, cc, t, n_tile, planes);
               if (++b_slot == p.b_slots) { b_slot = 0; b_phase ^= 1; }
             }
           }
@@ -312,7 +327,8 @@ static int halo_pick_ntiles(int m_tiles, int cout, int cchunks, int k16) {
 }
 
 // Host launcher shared by forward and stride-1 data gradient. `in` is the A-operand tensor [n,h,w,cin_ext] (pitch in_ld),
-// w is [cout][9][cin_ext] bf16. Returns B200SEG_E_BADARG when the shape is not eligible (caller falls back to the
+// w is [cout][9][cin_ext] bf16; w_planes (optional) the same weights as the plane-ordered image with planes_rows rows.
+// Returns B200SEG_E_BADARG when the shape is not eligible (caller falls back to the
 // generic per-tap kernel). The statistics partials are [grid][2][roundup16(cout)].
 // Tiling / shared-memory / occupancy decisions of one launch (host only; also reported by b200seg_conv2d_plan_info).
 static int halo_plan(int n, int h, int w, int cin, int cout, HaloParams& p, size_t& smem_bytes, int& grid, int& occ) {
@@ -375,10 +391,21 @@ static cudaError_t halo_set_attributes(HaloKernel k, int occ) {
 }
 
 int make_bn_fold(const b200seg_bn_fold* f, int cout, BnFoldDev* out);
+// Rows of the plane-ordered weight image of a Cout: the widest n_tiles x BN any halo plan of that Cout can ask for, so one
+// image serves every plan (the 0.5x and 1.0x passes of a layer may tile Cout differently).
+int conv3x3_halo_image_rows(int cout) {
+  int rows = 0;
+  for (int nt = 1; nt <= 16; ++nt) {
+    const int BN = ((cout + nt - 1) / nt + 15) / 16 * 16;
+    if (BN <= 256 && nt * BN > rows) rows = nt * BN;
+  }
+  return rows;
+}
+
 int conv3x3_halo_launch(int n, int h, int w, int cin, int in_ld, const void* in, int cout, const void* wts,
                         const float* bias, void* out, int out_ld, float* stats_partials, int32_t* stats_grid,
                         const void* addend, int addend_ld, int emit_stats, cudaStream_t stream,
-                        const b200seg_bn_fold* fold, const BnFoldDev* affine) {
+                        const b200seg_bn_fold* fold, const BnFoldDev* affine, const void* w_planes, int planes_rows) {
   if (in_ld % 8 || out_ld % 8) return B200SEG_E_BADARG;
   BnFoldDev fd;
   if (int frc = make_bn_fold(emit_stats ? fold : nullptr, cout, &fd)) return frc;
@@ -397,6 +424,12 @@ int conv3x3_halo_launch(int n, int h, int w, int cin, int in_ld, const void* in,
   if ((reinterpret_cast<uintptr_t>(in) & 15) || (reinterpret_cast<uintptr_t>(wts) & 15) ||
       (reinterpret_cast<uintptr_t>(out) & 15) || (reinterpret_cast<uintptr_t>(addend) & 15) || (addend && addend_ld % 8))
     return B200SEG_E_BADARG;
+  // the image: 16-byte aligned, and the last Cout tile's runs inside its rows
+  if (w_planes && ((reinterpret_cast<uintptr_t>(w_planes) & 15) || planes_rows < p.n_tiles * p.BN))
+    return B200SEG_E_BADARG;
+  p.w_planes = static_cast<const uint8_t*>(w_planes);
+  p.w_plane_bytes = (size_t)planes_rows * 16;
+  p.w_tap_bytes = (size_t)(cin + 15) / 16 * 2 * p.w_plane_bytes;
   CUtensorMap tmA, tmB;
   {   // one box = one 8-channel plane of the halo tile
     uint64_t dims[4] = {(uint64_t)cin, (uint64_t)w, (uint64_t)h, (uint64_t)n};

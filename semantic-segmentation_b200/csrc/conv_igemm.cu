@@ -512,8 +512,10 @@ void conv_igemm_occupancy_report() {
 int conv3x3_halo_launch(int n, int h, int w, int cin, int in_ld, const void* in, int cout, const void* wts,
                         const float* bias, void* out, int out_ld, float* stats_partials, int32_t* stats_grid,
                         const void* addend, int addend_ld, int emit_stats, cudaStream_t stream,
-                        const b200seg_bn_fold* fold = nullptr, const BnFoldDev* affine = nullptr);
+                        const b200seg_bn_fold* fold = nullptr, const BnFoldDev* affine = nullptr,
+                        const void* w_planes = nullptr, int planes_rows = 0);
 int conv3x3_halo_plan_info(int n, int h, int w, int cin, int cout, int32_t* out);
+int conv3x3_halo_image_rows(int cout);
 
 }  // namespace b200seg
 
@@ -553,6 +555,19 @@ extern "C" int b200seg_conv2d_plan_info(const b200seg_conv_desc* d, int32_t whic
   return 0;
 }
 
+// Plane-ordered weight image of the halo launch (which = 0 forward, 1 stride-1 data gradient): its bf16 element count and
+// rows, or 0 when that launch does not run on the halo kernel (it takes no image).
+extern "C" int64_t b200seg_conv2d_planes_elems(const b200seg_conv_desc* d, int32_t which, int32_t* rows) {
+  if (!desc_ok(d) || which < 0 || which > 1 || !halo_eligible(d, which)) {
+    if (rows) *rows = 0;
+    return 0;
+  }
+  const int cin = which == 0 ? d->cin : (d->cout + 7) / 8 * 8, cout = which == 0 ? d->cout : d->cin;
+  const int r = conv3x3_halo_image_rows(cout);
+  if (rows) *rows = r;
+  return (int64_t)9 * ((cin + 15) / 16 * 16) * r;
+}
+
 extern "C" int b200seg_conv2d_fwd(const b200seg_conv_desc* d, const void* x, const void* w_ohwi, const float* bias,
                                   void* y, float* stats_partials, int32_t* stats_grid, void* stream) {
   if (!desc_ok(d)) return B200SEG_E_BADARG;
@@ -560,7 +575,8 @@ extern "C" int b200seg_conv2d_fwd(const b200seg_conv_desc* d, const void* x, con
     if (d->emit_stats && !stats_partials) return B200SEG_E_BADARG;
     // halo-tile kernel: the input is read once per tile instead of once per filter tap (conv3x3_halo.cu)
     return conv3x3_halo_launch(d->n, d->h, d->w, d->cin, d->x_ld, x, d->cout, w_ohwi, d->has_bias ? bias : nullptr, y,
-                               d->y_ld, stats_partials, stats_grid, nullptr, 0, d->emit_stats, (cudaStream_t)stream);
+                               d->y_ld, stats_partials, stats_grid, nullptr, 0, d->emit_stats, (cudaStream_t)stream,
+                               nullptr, nullptr, d->w_planes, d->w_planes_rows);
   }
   return launch_geom(fwd_geom(d), x, w_ohwi, bias, y, stats_partials, stats_grid, nullptr, 0, (cudaStream_t)stream);
 }
@@ -576,7 +592,8 @@ extern "C" int b200seg_conv2d_fwd_bn(const b200seg_conv_desc* d, const void* x, 
   if (!desc_ok(d) || !fold || !d->emit_stats || d->out_fp32) return B200SEG_E_BADARG;
   if (halo_eligible(d, 0))
     return conv3x3_halo_launch(d->n, d->h, d->w, d->cin, d->x_ld, x, d->cout, w_ohwi, d->has_bias ? bias : nullptr, y,
-                               d->y_ld, nullptr, nullptr, nullptr, 0, 1, (cudaStream_t)stream, fold);
+                               d->y_ld, nullptr, nullptr, nullptr, 0, 1, (cudaStream_t)stream, fold, nullptr,
+                               d->w_planes, d->w_planes_rows);
   return launch_geom(fwd_geom(d), x, w_ohwi, bias, y, nullptr, nullptr, nullptr, 0, (cudaStream_t)stream, fold);
 }
 
@@ -590,7 +607,8 @@ extern "C" int b200seg_conv2d_fwd_add(const b200seg_conv_desc* d, const void* x,
   if (d->emit_stats && !stats_partials) return B200SEG_E_BADARG;
   if (halo_eligible(d, 0))
     return conv3x3_halo_launch(d->n, d->h, d->w, d->cin, d->x_ld, x, d->cout, w_ohwi, d->has_bias ? bias : nullptr, y,
-                               d->y_ld, stats_partials, stats_grid, addend, addend_ld, d->emit_stats, (cudaStream_t)stream);
+                               d->y_ld, stats_partials, stats_grid, addend, addend_ld, d->emit_stats, (cudaStream_t)stream,
+                               nullptr, nullptr, d->w_planes, d->w_planes_rows);
   return launch_geom(fwd_geom(d), x, w_ohwi, bias, y, stats_partials, stats_grid, addend, addend_ld, (cudaStream_t)stream);
 }
 
@@ -607,7 +625,8 @@ extern "C" int b200seg_conv2d_fwd_affine(const b200seg_conv_desc* d, const void*
   fd.relu = relu ? 1 : 0;
   if (halo_eligible(d, 0))
     return conv3x3_halo_launch(d->n, d->h, d->w, d->cin, d->x_ld, x, d->cout, w_ohwi, nullptr, y, d->y_ld, nullptr,
-                               nullptr, addend, addend_ld, 0, (cudaStream_t)stream, nullptr, &fd);
+                               nullptr, addend, addend_ld, 0, (cudaStream_t)stream, nullptr, &fd, d->w_planes,
+                               d->w_planes_rows);
   return launch_geom(fwd_geom(d), x, w_ohwi, nullptr, y, nullptr, nullptr, addend, addend_ld, (cudaStream_t)stream,
                      nullptr, &fd);
 }
@@ -630,7 +649,8 @@ extern "C" int b200seg_conv2d_dgrad(const b200seg_conv_desc* d, const void* dy, 
   g.out_fp32 = 0; g.has_bias = 0; g.emit_stats = 0; g.force_kc = d->reserved;
   if (halo_eligible(d, 1))
     return conv3x3_halo_launch(d->n, d->h, d->w, g.in_c, dy_ld, dy, d->cin, w_dgrad, nullptr, dx, dx_ld, nullptr, nullptr,
-                               addend, addend_ld, 0, (cudaStream_t)stream);
+                               addend, addend_ld, 0, (cudaStream_t)stream, nullptr, nullptr, d->w_planes,
+                               d->w_planes_rows);
   if (d->stride == 1) {
     g.sub_h = d->h; g.sub_w = d->w; g.out_stride = 1; g.out_off_h = g.out_off_w = 0;
     g.ntaps = taps;

@@ -27,17 +27,22 @@ __global__ void pack_weight_kernel(const float* __restrict__ w, int O, int I, in
 }
 
 // All weights of the model in ONE launch: block b repacks kPackChunk consecutive OIHW elements of item blk_item[b]
-// (fp32 master -> bf16 forward operand [O][taps][I_dst] and data-gradient operand [I_dst][taps flipped][o_pad]).
+// (fp32 master -> bf16 forward operand [O][taps][I_dst] and data-gradient operand [I_dst][taps flipped][o_pad], and the
+// plane-ordered images of both when planes[blk_item[b]] names them).
 constexpr int kPackChunk = 4096;
 __global__ void __launch_bounds__(256)
-pack_weights_kernel(const b200seg_pack_item* __restrict__ items, const int32_t* __restrict__ blk_item,
-                    const int32_t* __restrict__ blk_start, int which) {
+pack_weights_kernel(const b200seg_pack_item* __restrict__ items, const b200seg_pack_planes* __restrict__ planes,
+                    const int32_t* __restrict__ blk_item, const int32_t* __restrict__ blk_start, int which) {
   pdl_wait();     // no programmatic trigger: see pack_weight_kernel
   const b200seg_pack_item it = items[blk_item[blockIdx.x]];
+  const b200seg_pack_planes pl = planes ? planes[blk_item[blockIdx.x]] : b200seg_pack_planes{nullptr, nullptr, 0, 0};
   const float* __restrict__ w = reinterpret_cast<const float*>(it.w_oihw);
   __nv_bfloat16* __restrict__ ohwi = (which & 1) ? reinterpret_cast<__nv_bfloat16*>(it.w_ohwi) : nullptr;
   __nv_bfloat16* __restrict__ dgrad = (which & 2) ? reinterpret_cast<__nv_bfloat16*>(it.w_dgrad) : nullptr;
+  __nv_bfloat16* __restrict__ pf = (which & 1) ? reinterpret_cast<__nv_bfloat16*>(pl.fwd) : nullptr;
+  __nv_bfloat16* __restrict__ pd = (which & 2) ? reinterpret_cast<__nv_bfloat16*>(pl.dgrad) : nullptr;
   const uint32_t taps = (uint32_t)(it.ksize * it.ksize), I = (uint32_t)it.i, Id = (uint32_t)it.i_dst;
+  const uint32_t g_fwd = (Id + 15) / 16 * 2, g_dgrad = ((uint32_t)it.o + 15) / 16 * 2;   // planes per tap
   const uint32_t total = (uint32_t)it.o * I * taps;
   const uint32_t j0 = (uint32_t)blk_start[blockIdx.x];
 #pragma unroll 4
@@ -50,6 +55,9 @@ pack_weights_kernel(const b200seg_pack_item* __restrict__ items, const int32_t* 
     const __nv_bfloat16 v = __float2bfloat16_rn(w[idx]);
     if (ohwi) ohwi[((size_t)o * taps + t) * Id + i] = v;
     if (dgrad) dgrad[((size_t)i * taps + (taps - 1 - t)) * it.o_pad + o] = v;
+    // plane-ordered images (include/b200seg.h): [tap][Cin / 8][rows][8]
+    if (pf) pf[(((size_t)t * g_fwd + i / 8) * pl.rows_fwd + o) * 8 + i % 8] = v;
+    if (pd) pd[(((size_t)(taps - 1 - t) * g_dgrad + o / 8) * pl.rows_dgrad + i) * 8 + o % 8] = v;
   }
   __threadfence();
 }
@@ -63,8 +71,17 @@ extern "C" int32_t b200seg_pack_chunk(void) { return kPackChunk; }
 extern "C" int b200seg_pack_weights(const b200seg_pack_item* items, const int32_t* blk_item, const int32_t* blk_start,
                                     int32_t n_blocks, int32_t which, void* stream) {
   if (!items || !blk_item || !blk_start || n_blocks <= 0 || which < 1 || which > 3) return B200SEG_E_BADARG;
-  cudaError_t e = launch_k(pack_weights_kernel, dim3(n_blocks), dim3(256), 0, (cudaStream_t)stream, items, blk_item,
-                           blk_start, (int)which);
+  cudaError_t e = launch_k(pack_weights_kernel, dim3(n_blocks), dim3(256), 0, (cudaStream_t)stream, items,
+                           (const b200seg_pack_planes*)nullptr, blk_item, blk_start, (int)which);
+  return e == cudaSuccess ? 0 : (int)e;
+}
+
+extern "C" int b200seg_pack_weights_planes(const b200seg_pack_item* items, const b200seg_pack_planes* planes,
+                                           const int32_t* blk_item, const int32_t* blk_start, int32_t n_blocks,
+                                           int32_t which, void* stream) {
+  if (!items || !planes || !blk_item || !blk_start || n_blocks <= 0 || which < 1 || which > 3) return B200SEG_E_BADARG;
+  cudaError_t e = launch_k(pack_weights_kernel, dim3(n_blocks), dim3(256), 0, (cudaStream_t)stream, items, planes,
+                           blk_item, blk_start, (int)which);
   return e == cudaSuccess ? 0 : (int)e;
 }
 

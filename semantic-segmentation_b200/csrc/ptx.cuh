@@ -111,6 +111,12 @@ __device__ __forceinline__ void tma_load_4d(const CUtensorMap* m, uint64_t* bar,
       "r"(c3)
       : "memory");
 }
+// 1-D bulk copy of `bytes` contiguous bytes (a multiple of 16; both addresses 16-byte aligned), signalled on bar
+__device__ __forceinline__ void bulk_load(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
+}
 
 // shared -> global tile store (TMA): the box is clipped against the tensor extent, so edge tiles need no predication
 __device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* src, int c0, int c1, int c2, int c3) {

@@ -6,9 +6,10 @@ data sheet), then the launch-weighted total per step. Bytes are the sizes of the
 tools/trace_step.py counts them. Shapes and counts come from that tool's recorder (meta tensors, no device) in a child
 `python -O`; each shape is timed with tools/gpu_wgrad_bench.py's CUDA-graph replay on random bf16 inputs. The card's
 name, power limit and maximum SM clock are read in the same run. B200SEG_LIB_VARIANT=<tag> times
-lib/libb200seg_<tag>.so (see b200seg/_lib.py).
+lib/libb200seg_<tag>.so (see b200seg/_lib.py). --planes hands every halo launch a plane-ordered weight image (random
+bf16, include/b200seg.h), as the training and evaluation steps do.
 
-    python tools/gpu_conv_bench.py [--arch ocrnet.HRNet_Mscale] [--height 1024 --width 2048] [--out conv.json]"""
+    python tools/gpu_conv_bench.py [--arch ocrnet.HRNet_Mscale] [--height 1024 --width 2048] [--planes] [--out conv.json]"""
 import argparse
 import ctypes
 import importlib.util
@@ -114,6 +115,7 @@ def main():
     ap.add_argument("--width", type=int, default=2048)
     ap.add_argument("--launches", type=int, default=20, help="launches per CUDA-graph replay")
     ap.add_argument("--reps", type=int, default=5, help="timed replays per shape (the median is kept)")
+    ap.add_argument("--planes", action="store_true", help="halo launches stream their weights from the image")
     ap.add_argument("--out", default=None, help="also write the table as JSON")
     ap.add_argument("--trace-only", action="store_true", help=argparse.SUPPRESS)
     args = ap.parse_args()
@@ -135,7 +137,8 @@ def main():
         sys.exit("needs a CUDA device")
     L = _lib.lib()
     name, power, sm_clock = WB.card()
-    print("%s, power limit %s, max SM clock %s; library %s" % (name, power, sm_clock, os.path.basename(_lib.LIB_PATH)))
+    print("%s, power limit %s, max SM clock %s; library %s%s" % (name, power, sm_clock, os.path.basename(_lib.LIB_PATH),
+                                                             ", weight images" if args.planes else ""))
     print("%-12s %-34s %5s %-14s %9s %8s %8s %7s %10s" % ("entry", "shape (HxW cin->cout kK sS)", "calls",
                                                          "kern BN occ", "us", "TFLOP/s", "GB/s", "roof", "us/step"))
     rows, total_us, total_flop, total_roof = [], 0.0, 0.0, 0.0
@@ -149,6 +152,12 @@ def main():
         if L.b200seg_conv2d_plan_info(ctypes.byref(pd), which, plan) != 0:
             plan[0] = plan[1] = plan[6] = -1    # stride-2 data gradients: four sub-lattice launches, no plan query
         launch, keep = make_launch(L, entry, d, tuple(opt), torch)
+        if args.planes and plan[0] == 1:
+            img_rows = ctypes.c_int32(0)
+            n_img = L.b200seg_conv2d_planes_elems(ctypes.byref(d), which, ctypes.byref(img_rows))
+            img = (torch.randn(n_img, device="cuda") * 0.5).to(torch.bfloat16)
+            d.w_planes, d.w_planes_rows = img.data_ptr(), img_rows.value
+            keep = keep + (img,)
         us, times = WB.time_replay(launch, args.launches, args.reps)
         roof_us = max(flop / (PEAK_TFLOPS * 1e12), nbytes / (PEAK_GBS * 1e9)) * 1e6
         label = "%dx%d c%d->%d k%d s%d" % (d.h, d.w, d.cin, d.cout, d.ksize, d.stride)

@@ -4,8 +4,10 @@
 // {64 channels, 1 tap, BN rows} box, 128-byte swizzle); one consumer warp releases each slot as soon as it has landed, so
 // the loop runs at the rate the memory system delivers. With multicast each CTA of a 2-CTA cluster issues half of every
 // tile to both CTAs (halo: four planes; igemm: BN / 2 rows) and a slot is refilled once both CTAs have released it.
+// planes: the halo tile from the plane-ordered weight image ([tap][Cin/8][Cout rows][8], include/b200seg.h), one 1-D
+// cp.async.bulk of BN x 16 contiguous bytes per plane into the same shared-memory image as the halo boxes.
 // Built and run by tools/gpu_l2_fill_bench.py:
-//   l2_fill_bench <halo|igemm> <cin> <cout> <BN> <CTAs per SM> <multicast 0|1> <tiles per CTA>
+//   l2_fill_bench <halo|igemm|planes> <cin> <cout> <BN> <CTAs per SM> <multicast 0|1> <tiles per CTA> [ring slots]
 // prints one JSON line.
 #include <cstdio>
 #include <cstdlib>
@@ -16,7 +18,7 @@
 using namespace b200seg;
 
 struct FillParams {
-  int halo, cin, BN, n_tiles, k_tiles, slots, tile_bytes, iters, multicast;
+  int halo, planes, cin, BN, n_tiles, k_tiles, slots, tile_bytes, iters, multicast, cout_rows;
 };
 
 // ---------------------------------------------------------------- 2-CTA clusters (valid in a launch without clusters too)
@@ -47,7 +49,8 @@ __device__ __forceinline__ void load_3d(const CUtensorMap* m, uint64_t* bar, voi
     tma_load_3d(m, bar, dst, c0, c1, c2);
 }
 
-__global__ void __launch_bounds__(64) l2_fill_kernel(const __grid_constant__ CUtensorMap tm, const FillParams p) {
+__global__ void __launch_bounds__(64) l2_fill_kernel(const __grid_constant__ CUtensorMap tm, const FillParams p,
+                                                      const uint8_t* __restrict__ image) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* ring = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full = reinterpret_cast<uint64_t*>(ring + (size_t)p.slots * p.tile_bytes);
@@ -67,7 +70,12 @@ __global__ void __launch_bounds__(64) l2_fill_kernel(const __grid_constant__ CUt
         mbar_wait(&empty[s], ((i / p.slots) & 1) ^ 1);
         mbar_arrive_expect_tx(&full[s], p.tile_bytes);
         uint8_t* dst = ring + (size_t)s * p.tile_bytes;
-        if (p.halo) {
+        if (p.planes) {
+          const int G = (p.cin + 63) / 64 * 8;   // the benchmark's image carries every plane of the last chunk
+          for (int j = 0; j < 8; ++j)
+            bulk_load(dst + j * p.BN * 16, image + ((size_t)(t * G + 8 * cc + j) * p.cout_rows + n0) * 16, p.BN * 16,
+                      &full[s]);
+        } else if (p.halo) {
           for (int j = p.multicast ? 4 * (int)rank : 0, je = p.multicast ? j + 4 : 8; j < je; ++j)
             load_3d(&tm, &full[s], dst + j * p.BN * 16, cc * 64 + 8 * j, t, n0, p.multicast);
         } else {
@@ -99,12 +107,14 @@ __global__ void __launch_bounds__(64) l2_fill_kernel(const __grid_constant__ CUt
   } while (0)
 
 int main(int argc, char** argv) {
-  if (argc != 8) {
-    fprintf(stderr, "usage: %s <halo|igemm> <cin> <cout> <BN> <ctas per SM> <multicast> <tiles per CTA>\n", argv[0]);
+  if (argc != 8 && argc != 9) {
+    fprintf(stderr, "usage: %s <halo|igemm|planes> <cin> <cout> <BN> <ctas per SM> <multicast> <tiles per CTA> [slots]\n",
+            argv[0]);
     return 2;
   }
   FillParams p{};
-  p.halo = strcmp(argv[1], "halo") == 0;
+  p.planes = strcmp(argv[1], "planes") == 0;
+  p.halo = p.planes || strcmp(argv[1], "halo") == 0;
   p.cin = atoi(argv[2]);
   const int cout = atoi(argv[3]), occ = atoi(argv[5]);
   p.BN = atoi(argv[4]);
@@ -117,8 +127,16 @@ int main(int argc, char** argv) {
   const size_t smem = occ == 2 ? 110 * 1024 : 200 * 1024;
   p.slots = (int)((smem - 1024 - 128) / p.tile_bytes);
   if (p.slots > 8) p.slots = 8;
+  if (argc == 9) p.slots = atoi(argv[8]);
+  if ((p.planes && (p.multicast || p.cin % 8)) || p.slots < 1 || (size_t)p.slots * p.tile_bytes + 1024 + 128 > smem) {
+    fprintf(stderr, "planes: no multicast and cin a multiple of 8; the ring must fit in shared memory\n");
+    return 2;
+  }
+  // plane image: Cout rows padded so that the last Cout tile's runs stay inside the allocation
+  p.cout_rows = p.n_tiles * p.BN;
   void* w = nullptr;
-  const size_t wbytes = (size_t)cout * taps * p.cin * 2;
+  const size_t wbytes =
+      p.planes ? (size_t)p.cout_rows * taps * ((p.cin + 63) / 64 * 64) * 2 : (size_t)cout * taps * p.cin * 2;
   CK(cudaMalloc(&w, wbytes));
   CK(cudaMemset(w, 0x3c, wbytes));
   CUtensorMap tm;
@@ -153,12 +171,13 @@ int main(int argc, char** argv) {
   cudaEvent_t e0, e1;
   CK(cudaEventCreate(&e0));
   CK(cudaEventCreate(&e1));
-  CK(cudaLaunchKernelEx(&cfg, l2_fill_kernel, tm, p));   // warm-up: brings the weights into L2
+  const uint8_t* image = p.planes ? static_cast<const uint8_t*>(w) : nullptr;
+  CK(cudaLaunchKernelEx(&cfg, l2_fill_kernel, tm, p, image));   // warm-up: brings the weights into L2
   CK(cudaDeviceSynchronize());
   float best = 1e30f;
   for (int r = 0; r < 5; ++r) {
     CK(cudaEventRecord(e0));
-    CK(cudaLaunchKernelEx(&cfg, l2_fill_kernel, tm, p));
+    CK(cudaLaunchKernelEx(&cfg, l2_fill_kernel, tm, p, image));
     CK(cudaEventRecord(e1));
     CK(cudaEventSynchronize(e1));
     float ms = 0;
@@ -175,7 +194,7 @@ int main(int argc, char** argv) {
          "\"grid\": %d, \"slots\": %d, \"tile_bytes\": %d, \"weight_bytes\": %zu, \"ms\": %.4f, "
          "\"smem_fill_TBps\": %.3f, \"l2_read_TBps\": %.3f, \"smem_fill_B_per_clk_per_sm\": %.2f, "
          "\"l2_read_B_per_clk_per_sm\": %.2f, \"max_sm_clock_mhz\": %d}\n",
-         p.halo ? "halo" : "igemm", p.cin, cout, p.BN, occ, p.multicast, grid, p.slots, p.tile_bytes, wbytes, best,
+         p.planes ? "planes" : p.halo ? "halo" : "igemm", p.cin, cout, p.BN, occ, p.multicast, grid, p.slots, p.tile_bytes, wbytes, best,
          smem_bytes / s / 1e12, l2_bytes / s / 1e12, smem_bytes / s / (clk_khz * 1e3) / sms,
          l2_bytes / s / (clk_khz * 1e3) / sms, clk_khz / 1000);
   CK(cudaFree(w));

@@ -218,6 +218,7 @@ class _EvalNet:
         self.n_scales = (0.5, 1.0, 2.0) if A.is_two_scale(net.arch) else None
         self._tensors = lambda: tensors
         self._packed = packed
+        self._planes = {}       # the weight images change which bytes a halo launch reads, not the launches
         self._eval_bn_params = lambda: eval_bn
         self._ensure_device_state = self._repack = lambda: None
 
