@@ -538,6 +538,35 @@ typedef struct b200seg_aug_color {
 int b200seg_aug_color_normalize(const b200seg_aug_color* c, const uint8_t* rgb, int32_t h, int32_t w,
                                 uint64_t* luma_sum_ws, float* out_chw, void* stream);
 
+/* RandAugment (datasets/randaugment.py, --rand_augment N,M) between the two calls above: the ops of augment_list() on the
+ * uint8 crop rgb [h][w][3] and its int64 label map, bit-exact with Pillow 12. Host side (draws, matrices, static LUTs):
+ * b200seg/augment.py. Every entry reads one buffer and writes another. */
+typedef struct b200seg_aug_affine_desc {
+  int32_t h, w;                /* crop size (input and output) */
+  int32_t bilinear;            /* image: 1 BILINEAR (Image.transform), 0 NEAREST (Image.rotate); labels are always NEAREST */
+  int32_t scale;               /* NEAREST source pixels: 1 from tab_x [w] / tab_y [h] (matrix without shear terms, Pillow's
+                                  ImagingScaleAffine; -1 = outside), 0 from the 16.16 matrix `fixed` (affine_fixed) */
+  int32_t fixed[6];            /* FIX(a0), FIX(a1), FIX(a2 + a0/2 + a1/2), FIX(a3), FIX(a4), FIX(a5 + a3/2 + a4/2) */
+  int32_t label_fill;          /* label outside the source (the image gets black) */
+  int32_t reserved;
+  double a[6];                 /* output -> input affine matrix (Image.transform's data), read by BILINEAR */
+} b200seg_aug_affine_desc;
+/* ShearX / ShearY / TranslateX / TranslateY / Rotate */
+int b200seg_aug_affine(const b200seg_aug_affine_desc* d, const uint8_t* src_rgb, const int64_t* src_label,
+                       const int32_t* tab_x, const int32_t* tab_y, uint8_t* out_rgb, int64_t* out_label, void* stream);
+/* AutoContrast (kind 0) / Equalize (kind 1): per-channel histogram of rgb [npix][3] into hist_ws (768 uint32, zeroed here)
+ * and the ImageOps LUT int32 [3][256] computed from it on the device (apply it with b200seg_aug_point) */
+int b200seg_aug_hist_lut(int32_t kind, const uint8_t* rgb, int64_t npix, uint32_t* hist_ws, int32_t* lut, void* stream);
+/* Image.point: out[p][c] = lut[c][src[p][c]], lut int32 [3][256] with values in 0..255 (Invert, Solarize, Posterize and the
+ * histogram LUTs) */
+int b200seg_aug_point(const uint8_t* src_rgb, int64_t npix, const int32_t* lut, uint8_t* out_rgb, void* stream);
+#define B200SEG_AUG_ENHANCE_BRIGHTNESS 0   /* Image.blend with black */
+#define B200SEG_AUG_ENHANCE_COLOR 1        /* Image.blend with the L conversion */
+#define B200SEG_AUG_ENHANCE_SHARPNESS 2    /* Image.blend with ImageFilter.SMOOTH (border pixels unchanged) */
+/* ImageEnhance.<kind>(img).enhance(factor) */
+int b200seg_aug_enhance(int32_t kind, float factor, const uint8_t* src_rgb, int32_t h, int32_t w, uint8_t* out_rgb,
+                        void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -69,6 +69,11 @@ class AugColor(ctypes.Structure):
                 ("mean", c_float * 3), ("std", c_float * 3)]
 
 
+class AugAffine(ctypes.Structure):
+    _fields_ = [(n, c_int32) for n in ("h", "w", "bilinear", "scale")] + [("fixed", c_int32 * 6), ("label_fill", c_int32),
+                                                                         ("reserved", c_int32), ("a", ctypes.c_double * 6)]
+
+
 # name -> (restype, argtypes). Must list every symbol include/b200seg.h declares (tests/test_abi.py checks this).
 V, I32, I64, F = c_void_p, c_int32, c_int64, c_float
 SIGNATURES = {
@@ -155,6 +160,10 @@ SIGNATURES = {
     "b200seg_accum_pred": (ctypes.c_int, [V, V, I32, I32, I32, I32, I32, I32, V]),
     "b200seg_aug_resize_crop": (ctypes.c_int, [ctypes.POINTER(AugGeom), V, V, V, V, V, V, V, V, V, V, V, V]),
     "b200seg_aug_color_normalize": (ctypes.c_int, [ctypes.POINTER(AugColor), V, I32, I32, V, V, V]),
+    "b200seg_aug_affine": (ctypes.c_int, [ctypes.POINTER(AugAffine), V, V, V, V, V, V, V]),
+    "b200seg_aug_hist_lut": (ctypes.c_int, [I32, V, I64, V, V, V]),
+    "b200seg_aug_point": (ctypes.c_int, [V, I64, V, V, V]),
+    "b200seg_aug_enhance": (ctypes.c_int, [I32, F, V, I32, I32, V, V]),
     "b200seg_argmax_hist": (ctypes.c_int, [V, I32, I32, I64, F, V, V, V, V, V]),
 }
 # test-only entry points (csrc/probe.h, libb200seg_test.so), not part of include/b200seg.h / the product library

@@ -7,7 +7,7 @@ import ctypes
 
 import torch
 
-from ._lib import AugColor, AugGeom, BnFold, ConvDesc, FuseDesc, MscaleDesc, check, lib, ptr, stream_ptr
+from ._lib import AugAffine, AugColor, AugGeom, BnFold, ConvDesc, FuseDesc, MscaleDesc, check, lib, ptr, stream_ptr
 
 BF16 = torch.bfloat16
 F32 = torch.float32
@@ -787,9 +787,18 @@ def augment(image_u8, mask_u8, p, t, id_lut, ignore_label, mean, std, out_image=
     rgb = _new((th, tw, 3), dtype=torch.uint8, device=dev)
     if out_label is None:
         out_label = _new((th, tw), dtype=torch.int64, device=dev)
+    ra_steps = t.get("ra")
+    label = out_label
+    if ra_steps:       # the geometric ops swap the label buffers: start in the one that makes the last swap end in out_label
+        spare = _new((th, tw), dtype=torch.int64, device=dev)
+        if sum(kind == "affine" for kind, _ in ra_steps) % 2:
+            label, spare = spare, label
     check(lib().b200seg_aug_resize_crop(ctypes.byref(g), ptr(image_u8), ptr(mask_u8), ptr(tab[0]), ptr(tab[1]),
                                         ptr(tab[2]), ptr(tab[3]), ptr(tab[4]), ptr(tab[5]), ptr(id_lut), ptr(rgb),
-                                        ptr(out_label), stream_ptr()), "aug_resize_crop")
+                                        ptr(label), stream_ptr()), "aug_resize_crop")
+    if ra_steps:
+        rgb, label = rand_augment(rgb, label, spare, ra_steps)
+        assert label.data_ptr() == out_label.data_ptr()
     c = AugColor()
     c.n_ops = len(p.ops)
     has_contrast = False
@@ -806,3 +815,50 @@ def augment(image_u8, mask_u8, p, t, id_lut, ignore_label, mean, std, out_image=
     check(lib().b200seg_aug_color_normalize(ctypes.byref(c), ptr(rgb), th, tw, ptr(ws), ptr(out_image), stream_ptr()),
           "aug_color_normalize", launches=2 if has_contrast else 1)
     return out_image, out_label, rgb
+
+
+def rand_augment(rgb, label, spare_label, steps):
+    """RandAugment's ops on the crop rgb uint8 [h,w,3] and its labels int64 [h,w], in order. steps: the host plan of
+    b200seg.augment.randaugment_steps. Pixels ping-pong between rgb and one more buffer, labels between label and
+    spare_label (geometric ops only). Returns the (rgb, label) buffers holding the result."""
+    import numpy as np
+    h, w = label.shape
+    npix = h * w
+    dev = rgb.device
+    L, stream = lib(), stream_ptr()
+    parts = []                # one upload for every NEAREST table and static LUT of the chain
+    for kind, s in steps:
+        if kind == "affine" and s["scale"]:
+            parts += [s["tab_x"], s["tab_y"]]
+        elif kind == "lut":
+            parts.append(s)
+    if parts:
+        flat = torch.from_numpy(np.concatenate(parts).astype(np.int32)).pin_memory().to(dev, non_blocking=True)
+    offs = np.cumsum([0] + [x.size for x in parts])
+    tabs = iter([flat[offs[i]:offs[i + 1]] for i in range(len(parts))])
+    if any(kind == "hist" for kind, _ in steps):
+        hist_ws = _new((768,), dtype=torch.int32, device=dev)
+        hist_lut = _new((768,), dtype=torch.int32, device=dev)
+    out = _new((h, w, 3), dtype=torch.uint8, device=dev)
+    for kind, s in steps:
+        if kind == "affine":
+            d = AugAffine()
+            d.h, d.w, d.bilinear, d.scale, d.label_fill = h, w, int(s["bilinear"]), int(s["scale"]), int(s["label_fill"])
+            for i in range(6):
+                d.a[i] = s["a"][i]
+                d.fixed[i] = s["fixed"][i] if not s["scale"] else 0
+            tx, ty = (next(tabs), next(tabs)) if s["scale"] else (None, None)
+            check(L.b200seg_aug_affine(ctypes.byref(d), ptr(rgb), ptr(label), ptr(tx), ptr(ty), ptr(out),
+                                       ptr(spare_label), stream), "aug_affine")
+            label, spare_label = spare_label, label
+        elif kind == "hist":
+            check(L.b200seg_aug_hist_lut(int(s), ptr(rgb), npix, ptr(hist_ws), ptr(hist_lut), stream), "aug_hist_lut",
+                  launches=2)
+            check(L.b200seg_aug_point(ptr(rgb), npix, ptr(hist_lut), ptr(out), stream), "aug_point")
+        elif kind == "lut":
+            check(L.b200seg_aug_point(ptr(rgb), npix, ptr(next(tabs)), ptr(out), stream), "aug_point")
+        else:
+            enhance, factor = s
+            check(L.b200seg_aug_enhance(int(enhance), float(factor), ptr(rgb), h, w, ptr(out), stream), "aug_enhance")
+        rgb, out = out, rgb
+    return rgb, label
